@@ -99,6 +99,9 @@ def lib():
             "ddpm_sampler_reset": ([vp, i32, vp], i32),
             "ddpm_sampler_step": ([vp, vp, vp, u64, vp], i32),
             "ddpm_sampler_step_pred": ([vp, vp, vp, u64, vp, vp], i32),
+            "ddpm_bpd_setup": ([vp, i32, vp], i32),
+            "ddpm_bpd_reset": ([vp, i32, vp], i32),
+            "ddpm_bpd_step": ([vp, vp, vp, i32, vp, vp, vp], i32),
             "ddpm_unet_grad_chunks": ([vp, i32, C.POINTER(i64), C.POINTER(i64)], i32),
             "ddpm_unet_wait_grad_chunk": ([vp, i32, vp], i32),
             "ddpm_unet_plan_stats": ([vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32),
@@ -120,7 +123,8 @@ EXPORTS = ["ddpm_last_error", "ddpm_runtime_check", "ddpm_device_error_flag", "d
            "ddpm_unet_create", "ddpm_unet_destroy", "ddpm_unet_num_params", "ddpm_unet_param_info",
            "ddpm_unet_flat_elems", "ddpm_unet_workspace_bytes", "ddpm_unet_plan", "ddpm_unet_repack",
            "ddpm_unet_forward", "ddpm_unet_backward", "ddpm_train_forward", "ddpm_train_backward",
-           "ddpm_sampler_setup", "ddpm_sampler_reset", "ddpm_sampler_step", "ddpm_sampler_step_pred", "ddpm_unet_grad_chunks", "ddpm_unet_wait_grad_chunk", "ddpm_unet_plan_stats",
+           "ddpm_sampler_setup", "ddpm_sampler_reset", "ddpm_sampler_step", "ddpm_sampler_step_pred",
+           "ddpm_bpd_setup", "ddpm_bpd_reset", "ddpm_bpd_step", "ddpm_unet_grad_chunks", "ddpm_unet_wait_grad_chunk", "ddpm_unet_plan_stats",
            "ddpm_unet_launches_per_forward", "ddpm_unet_launch_counts", "ddpm_opt_step", "ddpm_to_uint8_nhwc"]
 
 

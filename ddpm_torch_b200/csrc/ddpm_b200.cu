@@ -12,6 +12,9 @@ struct ddpm_unet {
     UnetEngine e;
     // sampler tables (device, owned by the handle; allocated by ddpm_sampler_setup, never per step)
     long long* d_tmodel = nullptr; float* d_coef = nullptr; int S = 0;
+    // bits/dim tables (allocated by ddpm_bpd_setup; separate from the sampler's, whose addresses a captured sampler graph holds):
+    // t_model i64[T] = 0..T-1, rows f32[T][kBpdRow], sqrt_ab f32[T], sqrt_1mab f32[T]
+    void* d_bpd = nullptr; int bpd_T = 0;
     const float* train_target = nullptr;
 };
 
@@ -86,6 +89,7 @@ void ddpm_unet_destroy(ddpm_unet* h) {
     if (!h) return;
     if (h->d_tmodel) cudaFree(h->d_tmodel);
     if (h->d_coef) cudaFree(h->d_coef);
+    if (h->d_bpd) cudaFree(h->d_bpd);
     if (h->e.side_stream) { cudaStreamSynchronize(h->e.side_stream);   // a queued weight re-pack still writes into the caller's workspace
         cudaStreamDestroy(h->e.side_stream); cudaEventDestroy(h->e.ev_fork); cudaEventDestroy(h->e.ev_join); }
     for (auto& c : h->e.chunks) if (c.ev) cudaEventDestroy(c.ev);
@@ -208,7 +212,7 @@ int ddpm_sampler_step_pred(ddpm_unet* h, float* x, const float* z, uint64_t seed
     UnetEngine& e = h->e;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     long long* tbuf = e.at<long long>(e.tbuf_off); float* cc = e.at<float>(e.coefcur_off); float* eps = e.at<float>(e.eps_off);
-    launch_k(k_sampler_prep, 1, 256, 0, st, e.at<int>(e.counter_off), h->d_tmodel, h->d_coef, tbuf, cc, e.B);
+    launch_k(k_sampler_prep, 1, 256, 0, st, e.at<int>(e.counter_off), h->d_tmodel, h->d_coef, 6, tbuf, cc, e.B);
     DDPM_CUDA_OK(cudaGetLastError());
     e.x_in = x; e.t_in = tbuf; e.eps_dst = eps; e.drop_seed = 0;
     static const bool no_uni = getenv("DDPM_NO_UNIFORM_T") != nullptr;
@@ -226,6 +230,76 @@ int ddpm_sampler_step_pred(ddpm_unet* h, float* x, const float* z, uint64_t seed
         launch_k(k_psample_tail, grid_for(total), 256, 0, st, eps, x, z, cc, (unsigned long long)seed, total, pred_x0);
         DDPM_CUDA_OK(cudaGetLastError());
     }
+    return 0;
+}
+
+int ddpm_bpd_setup(ddpm_unet* h, int T, const float* coef_host) {
+    if (!h || !coef_host) return fail(-30, "ddpm_bpd_setup: null argument");
+    if (T <= 0 || T > (1 << 24)) return fail(-30, "ddpm_bpd_setup: T must be in 1..2^24 (the step index travels as a float)");
+    const size_t bytes = (size_t)T * 8 + (size_t)T * (kBpdRow + 2) * 4;
+    std::vector<uint8_t> host(bytes);
+    long long* tm = reinterpret_cast<long long*>(host.data());
+    float* rows = reinterpret_cast<float*>(tm + T); float* ta = rows + (size_t)T * kBpdRow; float* ts = ta + T;
+    for (int i = 0; i < T; ++i) {
+        tm[i] = i;
+        for (int k = 0; k < kBpdRow; ++k) rows[(size_t)i * kBpdRow + k] = coef_host[(size_t)i * kBpdRow + k];
+        ta[i] = coef_host[(size_t)i * kBpdRow + 0];       // the q_sample prologue indexes its tables by t
+        ts[i] = coef_host[(size_t)i * kBpdRow + 1];
+    }
+    if (h->bpd_T != T) {       // same length: keep the allocation (a captured bits/dim graph holds its address)
+        if (h->d_bpd) { cudaFree(h->d_bpd); h->d_bpd = nullptr; h->bpd_T = 0; }
+        DDPM_CUDA_OK(cudaMalloc(&h->d_bpd, bytes));
+    }
+    DDPM_CUDA_OK(cudaMemcpy(h->d_bpd, host.data(), bytes, cudaMemcpyHostToDevice));
+    h->bpd_T = T;
+    return 0;
+}
+int ddpm_bpd_reset(ddpm_unet* h, int first_step, void* stream) {
+    NEED_PLAN(h);
+    if (!h->d_bpd) return fail(-33, "ddpm_bpd_setup has not been called");
+    if (first_step < 0 || first_step >= h->bpd_T) return fail(-30, "first_step out of range");
+    launch_k(k_set_int, 1, 1, 0, static_cast<cudaStream_t>(stream), h->e.at<int>(h->e.counter_off), first_step);
+    DDPM_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+int ddpm_bpd_step(ddpm_unet* h, const float* x0, const float* noise, int clip_denoised, float* losses, float* mses, void* stream) {
+    if (!h) return fail(-30, "ddpm_bpd_step: null handle");
+    if (!x0 || !noise || !losses || !mses) return fail(-30, "ddpm_bpd_step: null buffer");
+    NEED_PLAN(h);
+    if (!h->d_bpd) return fail(-33, "ddpm_bpd_setup has not been called");
+    UnetEngine& e = h->e;
+    const int Cin = e.cfg.in_channels, Cout = e.cfg.out_channels, HW = e.H * e.W, T = h->bpd_T;
+    if (Cin != Cout) return fail(-30, "ddpm_bpd_step: eps prediction needs out_channels == in_channels");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const long long* tm = static_cast<const long long*>(h->d_bpd);
+    const float* rows = reinterpret_cast<const float*>(tm + T); const float* ta = rows + (size_t)T * kBpdRow; const float* ts = ta + T;
+    long long* tbuf = e.at<long long>(e.tbuf_off); float* cc = e.at<float>(e.coefcur_off);
+    float* xt = e.at<float>(e.xt_off); float* eps = e.at<float>(e.eps_off); float* part = e.at<float>(e.bpd_part_off);
+    launch_k(k_sampler_prep, 1, 256, 0, st, e.at<int>(e.counter_off), tm, rows, kBpdRow, tbuf, cc, e.B);
+    DDPM_CUDA_OK(cudaGetLastError());
+    // x_t = q_sample(x_0, t, noise) (diffusion.py:92-97) is formed in in_conv's loads and stored once to xt; the plain
+    // forward follows (no one-row timestep path), so eps equals what ddpm_unet_forward(x_t, t) computes
+    e.qs_pro = QsamplePro{noise, tbuf, ta, ts, xt};
+    e.x_in = x0; e.t_in = tbuf; e.eps_dst = eps; e.drop_seed = 0;
+    const BpdEpi bp{x0, xt, cc, part, clip_denoised ? 1 : 0};
+    const bool fused = e.gather_fused_tail;
+    if (fused) e.bpd_epi = bp;                         // eps never reaches memory
+    const int rc = e.run_list(e.fwd_ops, st);
+    e.qs_pro = QsamplePro{};
+    e.bpd_epi = BpdEpi{};
+    if (rc) return rc;
+    const int nbi = (HW + 255) / 256;
+    if (!fused) {
+        switch (Cout) {
+            case 1: launch_k(k_bpd_tail<1>, e.B * nbi, 256, 0, st, (const float*)eps, bp, HW); break;
+            case 2: launch_k(k_bpd_tail<2>, e.B * nbi, 256, 0, st, (const float*)eps, bp, HW); break;
+            case 3: launch_k(k_bpd_tail<3>, e.B * nbi, 256, 0, st, (const float*)eps, bp, HW); break;
+            default: launch_k(k_bpd_tail<4>, e.B * nbi, 256, 0, st, (const float*)eps, bp, HW); break;
+        }
+        DDPM_CUDA_OK(cudaGetLastError());
+    }
+    launch_k(k_bpd_finalize, 1, 256, 0, st, (const float*)part, nbi, e.B, (float)(Cout * HW), (const float*)cc, T, losses, mses);
+    DDPM_CUDA_OK(cudaGetLastError());
     return 0;
 }
 int ddpm_opt_step(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, float* ema_shadow, long long n,

@@ -78,6 +78,78 @@ __device__ __forceinline__ float psample_update(float xt, float eps, float zz, f
     const float mean = __fadd_rn(__fmul_rn(c2, x0), __fmul_rn(c3, xt));
     return __fadd_rn(mean, __fmul_rn(nzsg, zz));
 }
+
+// Bits/dim epilogue of the final conv (GaussianDiffusion.calc_all_bpd, diffusion.py:107-138,203-215; functions.py:28-64).
+// With `bp.part` set, k_out_gather (or k_bpd_tail, for plans whose out_conv is not on the tensor cores) turns eps into the
+// variational-bound term and the squared x_0 error of every element and writes per-block partial sums; k_bpd_finalize adds
+// them in a fixed order (no floating-point atomics).  Blocks never straddle images: block j of image b owns pixels
+// [256 j, 256 j + 256) of that image, so the grid is B * ceil(H*W / 256).
+// Per-step row (ddpm_bpd_setup): {sqrt_ab, sqrt_1mab, sqrt_recip_ab, sqrt_recip_m1_ab, post_c1, post_c2, model_logvar,
+// true_logvar, t>0}; k_sampler_prep appends the step index.
+constexpr int kBpdRow = 9;
+struct BpdEpi { const float* x0; const float* xt; const float* coef; float* part /*[B*nbi][2]*/; int clip; };
+struct BpdCoef { float ra, rm1, pc1, pc2, a /*-1 - d*/, em /*exp(-lv_model)*/, ed /*exp(d)*/, inv_std; bool kl; };
+// per-step scalars, formed as the torch expressions form their [B,1,1,1] operands
+__device__ __forceinline__ BpdCoef bpd_coef(const float* c) {
+    BpdCoef k;
+    k.ra = c[2]; k.rm1 = c[3]; k.pc1 = c[4]; k.pc2 = c[5];
+    const float lvm = c[6], d = __fsub_rn(c[7], lvm);
+    k.a = __fsub_rn(-1.f, d); k.em = expf(-lvm); k.ed = expf(d);
+    k.inv_std = expf(-__fmul_rn(0.5f, lvm));
+    k.kl = c[8] != 0.f;
+    return k;
+}
+// functions.py:38-44: 0.5 * (1 + tanh(sqrt(2/pi) * (x + 0.044715 * x^3)))
+__device__ __forceinline__ float approx_std_normal_cdf(float x) {
+    const float x3 = __fmul_rn(__fmul_rn(x, x), x);
+    const float in = __fadd_rn(x, __fmul_rn(0.044715f, x3));
+    return __fmul_rn(0.5f, __fadd_rn(1.f, tanhf(__fmul_rn(0.7978845608028654f, in))));
+}
+// One element: term = KL(q(x_{t-1}|x_t,x_0) || p(x_{t-1}|x_t)) for t > 0, else the discretised decoder NLL; sq = (pred - x_0)^2.
+// Every operation is a separately rounded fp32 op in the mirror's operand order, so given the same eps an element equals
+// what the torch formulas compute.
+__device__ __forceinline__ void bpd_elem(float xt, float x0, float eps, const BpdCoef& k, int clip, float& term, float& sq) {
+    float pred = __fsub_rn(__fmul_rn(k.ra, xt), __fmul_rn(k.rm1, eps));
+    if (clip) pred = fminf(fmaxf(pred, -1.f), 1.f);
+    const float mm = __fadd_rn(__fmul_rn(k.pc1, pred), __fmul_rn(k.pc2, xt));
+    if (k.kl) {
+        const float mt = __fadd_rn(__fmul_rn(k.pc1, x0), __fmul_rn(k.pc2, xt));
+        const float dm = __fsub_rn(mt, mm);
+        term = __fmul_rn(__fadd_rn(__fadd_rn(k.a, __fmul_rn(__fmul_rn(dm, dm), k.em)), k.ed), 0.5f);
+    } else {
+        const float c = __fsub_rn(x0, mm);
+        const float hi = x0 > 0.999f ? 1.f : approx_std_normal_cdf(__fmul_rn(k.inv_std, __fadd_rn(c, 1.f / 255.f)));
+        const float lo = x0 < -0.999f ? 0.f : approx_std_normal_cdf(__fmul_rn(k.inv_std, __fsub_rn(c, 1.f / 255.f)));
+        term = -logf(__fadd_rn(fmaxf(__fsub_rn(__fsub_rn(hi, lo), 1e-12f), 0.f), 1e-12f));
+    }
+    const float e = __fsub_rn(pred, x0);
+    sq = __fmul_rn(e, e);
+}
+// the CO channels of pixel p of image b, eps given
+template <int CO>
+__device__ __forceinline__ void bpd_pixel(const BpdEpi& bp, const BpdCoef& k, const float (&eps)[CO], long long b, int p, int HW,
+                                          float& term, float& sq) {
+#pragma unroll
+    for (int co = 0; co < CO; ++co) {
+        const long long j = (b * CO + co) * HW + p;
+        float t_, s_;
+        bpd_elem(__ldg(bp.xt + j), __ldg(bp.x0 + j), eps[co], k, bp.clip, t_, s_);
+        term = __fadd_rn(term, t_); sq = __fadd_rn(sq, s_);
+    }
+}
+// block sum of (term, sq) -> part[blockIdx.x]; every thread of the block must call it (blockDim.x == 256)
+__device__ __forceinline__ void bpd_block_partial(float term, float sq, float* part) {
+    __shared__ float red[2][8];
+    term = warp_sum(term); sq = warp_sum(sq);
+    const int w = threadIdx.x >> 5;
+    if ((threadIdx.x & 31) == 0) { red[0][w] = term; red[1][w] = sq; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float a = 0.f, s = 0.f;
+        for (int i = 0; i < 8; ++i) { a += red[0][i]; s += red[1][i]; }
+        part[2 * blockIdx.x] = a; part[2 * blockIdx.x + 1] = s;
+    }
+}
 __device__ __forceinline__ float philox_normal(unsigned long long seed, uint32_t step, long long i) {
     const uint4 r = philox4x32((uint32_t)i, (uint32_t)(i >> 32), (uint32_t)seed ^ (step * 0x9E3779B1u), (uint32_t)(seed >> 32));
     const float u1 = ((float)r.x + 1.f) * 2.3283064365386963e-10f, u2 = (float)r.y * 2.3283064365386963e-10f;
@@ -1316,6 +1388,37 @@ __global__ void k_psample_tail(const float* __restrict__ eps, float* __restrict_
         x[i] = psample_update(x[i], eps[i], zz, c0, c1, c2, c3, nzsg, pred ? pred + i : nullptr);
     }
 }
+// bits/dim tail for plans without the fused gather: eps f32[B][CO][H][W] from memory, same block layout and arithmetic as the
+// BpdEpi path of k_out_gather.  grid = B * ceil(H*W / 256), block = 256.
+template <int CO>
+__global__ void __launch_bounds__(256) k_bpd_tail(const float* __restrict__ eps, const BpdEpi bp, int HW) {
+    pdl_entry();
+    const int nbi = (HW + 255) / 256;
+    const long long b = blockIdx.x / nbi;
+    const int p = (blockIdx.x % nbi) * 256 + threadIdx.x;
+    const BpdCoef k = bpd_coef(bp.coef);
+    float term = 0.f, sq = 0.f;
+    if (p < HW) {
+        float e[CO];
+#pragma unroll
+        for (int co = 0; co < CO; ++co) e[co] = __ldg(eps + (b * CO + co) * HW + p);
+        bpd_pixel<CO>(bp, k, e, b, p, HW, term, sq);
+    }
+    bpd_block_partial(term, sq, bp.part);
+}
+// fixed-order sum of the nbi partials of each image: losses[b][ti] = mean(term) / ln 2, mses[b][ti] = mean(sq), with
+// ti = the step index k_sampler_prep stored behind the coefficient row
+__global__ void k_bpd_finalize(const float* __restrict__ part, int nbi, int B, float n, const float* __restrict__ coef, int T,
+                               float* __restrict__ losses, float* __restrict__ mses) {
+    pdl_entry();
+    const int ti = (int)coef[kBpdRow];
+    for (int b = threadIdx.x; b < B; b += blockDim.x) {
+        float a = 0.f, s = 0.f;
+        for (int j = 0; j < nbi; ++j) { a += part[2 * (b * nbi + j)]; s += part[2 * (b * nbi + j) + 1]; }
+        losses[(long long)b * T + ti] = a / n / 0.6931471805599453f;
+        mses[(long long)b * T + ti] = s / n;
+    }
+}
 // generate.py:129  (x * 127.5 + 127.5).round().clamp(0, 255).to(uint8).permute(0, 2, 3, 1): NCHW fp32 -> NHWC uint8.
 // Bit-exact with the reference expression: separate fp32 multiply and add (no FMA contraction), round-half-to-even.
 template <int C>
@@ -1413,25 +1516,45 @@ __global__ void k_unpack_tap(const float* __restrict__ S, float* __restrict__ gw
     gw[i] = mode == 0 ? S[(long long)(t * CO + co) * CI + ci] : S[(long long)co * 64 + t * CI + ci];
 }
 template <int CO>
+__device__ __forceinline__ void out_gather_px(const float* __restrict__ T, const float* __restrict__ bias, long long b, int y, int x, int H, int W,
+                                              float (&acc)[CO]) {
+#pragma unroll
+    for (int co = 0; co < CO; ++co) acc[co] = bias ? __ldg(bias + co) : 0.f;
+#pragma unroll
+    for (int t = 0; t < 9; ++t) {
+        const int yy = y + t / 3 - 1, xx = x + t % 3 - 1;
+        if (yy < 0 || yy >= H || xx < 0 || xx >= W) continue;
+        const float* r = T + ((b * H + yy) * W + xx) * 32 + t * CO;
+#pragma unroll
+        for (int co = 0; co < CO; ++co) acc[co] += __ldg(r + co);
+    }
+}
+// With bp.part set the launch grid is B * ceil(H*W / 256) (the bits/dim block layout) instead of a grid-stride loop.
+template <int CO>
 __global__ void __launch_bounds__(256) k_out_gather(const float* __restrict__ T /*[P][32]*/, const float* __restrict__ bias, float* __restrict__ out /*NCHW*/,
-                                                   int B, int H, int W, const PsampleEpi ps) {
+                                                   int B, int H, int W, const PsampleEpi ps, const BpdEpi bp) {
     pdl_entry();
+    if (bp.part) {
+        const int HW = H * W, nbi = (HW + 255) / 256;
+        const long long b = blockIdx.x / nbi;
+        const int p = (blockIdx.x % nbi) * 256 + threadIdx.x;
+        const BpdCoef k = bpd_coef(bp.coef);
+        float term = 0.f, sq = 0.f;
+        if (p < HW) {
+            float acc[CO];
+            out_gather_px<CO>(T, bias, b, p / W, p % W, H, W, acc);
+            bpd_pixel<CO>(bp, k, acc, b, p, HW, term, sq);
+        }
+        bpd_block_partial(term, sq, bp.part);
+        return;
+    }
     const long long P = (long long)B * H * W;
     float c0 = 0.f, c1 = 0.f, c2 = 0.f, c3 = 0.f, nzsg = 0.f; uint32_t step = 0;
     if (ps.x) { c0 = ps.coef[0]; c1 = ps.coef[1]; c2 = ps.coef[2]; c3 = ps.coef[3]; nzsg = __fmul_rn(ps.coef[5], ps.coef[4]); step = (uint32_t)ps.coef[6]; }
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < P; i += (long long)gridDim.x * blockDim.x) {
         const int x = (int)(i % W), y = (int)((i / W) % H); const long long b = i / ((long long)W * H);
         float acc[CO];
-#pragma unroll
-        for (int co = 0; co < CO; ++co) acc[co] = bias ? __ldg(bias + co) : 0.f;
-#pragma unroll
-        for (int t = 0; t < 9; ++t) {
-            const int yy = y + t / 3 - 1, xx = x + t % 3 - 1;
-            if (yy < 0 || yy >= H || xx < 0 || xx >= W) continue;
-            const float* r = T + ((b * H + yy) * W + xx) * 32 + t * CO;
-#pragma unroll
-            for (int co = 0; co < CO; ++co) acc[co] += __ldg(r + co);
-        }
+        out_gather_px<CO>(T, bias, b, y, x, H, W, acc);
         if (ps.x) {
 #pragma unroll
             for (int co = 0; co < CO; ++co) {
@@ -1494,14 +1617,15 @@ __global__ void k_bcast_rows(float4* __restrict__ m, long long row4, long long t
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < tot4) m[row4 + i] = m[i % row4];
 }
-// one block: fetch step i = *counter, broadcast t_model[i] to t_buf[B], copy the coefficient row, then advance the counter
-__global__ void k_sampler_prep(int* __restrict__ counter, const long long* __restrict__ t_model, const float* __restrict__ coef_table /*[S][6]*/,
-                               long long* __restrict__ t_buf, float* __restrict__ coef_cur /*[7]*/, int B) {
+// one block: fetch step i = *counter, broadcast t_model[i] to t_buf[B], copy the coefficient row (width floats; 6 for the
+// sampler, kBpdRow for bits/dim) followed by the step index, then advance the counter
+__global__ void k_sampler_prep(int* __restrict__ counter, const long long* __restrict__ t_model, const float* __restrict__ coef_table /*[S][width]*/,
+                               int width, long long* __restrict__ t_buf, float* __restrict__ coef_cur /*[width + 1]*/, int B) {
     pdl_entry();
     const int i = *counter;
     for (int b = threadIdx.x; b < B; b += blockDim.x) t_buf[b] = t_model[i];
-    if (threadIdx.x < 6) coef_cur[threadIdx.x] = coef_table[i * 6 + threadIdx.x];
-    if (threadIdx.x == 6) coef_cur[6] = (float)i;
+    if (threadIdx.x < width) coef_cur[threadIdx.x] = coef_table[i * width + threadIdx.x];
+    if (threadIdx.x == width) coef_cur[width] = (float)i;
     __syncthreads();
     if (threadIdx.x == 0) *counter = i - 1;
 }

@@ -67,6 +67,7 @@ struct UnetEngine {
     unsigned long long drop_seed = 0;
     // diffusion-side internal buffers
     size_t xt_off = 0, eps_off = 0, tbuf_off = 0, coefcur_off = 0, counter_off = 0, deps_off = 0;
+    size_t bpd_part_off = 0;               // bits/dim per-block partial sums [B * ceil(H*W/256)][2]
 
     // ------------------------------------------------------------------ parameters (reference registration order)
     void add_param(const std::string& n, std::initializer_list<int> d) {
@@ -326,7 +327,8 @@ struct UnetEngine {
     }
     float* eps_dst = nullptr;   // run-time destination of the final conv (caller buffer or internal eps buffer)
     PsampleEpi ps_epi = {nullptr, nullptr, nullptr, 0, nullptr};   // run-time: sampler update fused into the final gather (x != null)
-    QsamplePro qs_pro = {};           // run-time: q_sample fused into in_conv's loads (ddpm_train_forward)
+    QsamplePro qs_pro = {};           // run-time: q_sample fused into in_conv's loads (ddpm_train_forward, ddpm_bpd_step)
+    BpdEpi bpd_epi = {};              // run-time: bits/dim terms fused into the final gather (part != null; ddpm_bpd_step)
     bool gather_fused_tail = false;   // plan property: the final conv ends in k_out_gather (tensor-core out_conv path)
     const float* deps_src = nullptr;   // run-time d(loss)/d(eps), fp32 NCHW (caller buffer or internal buffer)
     int plan_error = 0;

@@ -19,6 +19,8 @@ def get_selection_schedule(schedule, size, timesteps):
 
 
 class DDIM(GaussianDiffusion):
+    _native_bpd = False           # calc_all_bpd over the sub-sequence tables keeps the generic formulas
+
     def __init__(self, betas, model_mean_type, model_var_type, loss_type, eta, subsequence):
         super().__init__(betas, model_mean_type, model_var_type, loss_type)
         self.eta = eta

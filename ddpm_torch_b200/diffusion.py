@@ -7,7 +7,9 @@ the configuration is the one every reference config uses (eps-prediction, fixed 
 * ``train_losses``  -> one fused engine call: q_sample prologue, UNet forward, per-sample MSE (and the matching
   fused backward through autograd),
 * ``p_sample`` / ``p_sample_step`` -> the engine's sampler step (UNet forward + the alpha/beta update of
-  diffusion.py:107-158 in one launch sequence, replayed from a CUDA graph once per timestep).
+  diffusion.py:107-158 in one launch sequence, replayed from a CUDA graph once per timestep),
+* ``calc_all_bpd`` -> the engine's bits/dim step (q_sample, UNet forward and the variational-bound terms of
+  diffusion.py:203-215 in one launch sequence, replayed from a CUDA graph once per timestep).
 
 Any other ``denoise_fn`` (toy MLPs, wrappers) takes the generic formulas below, written with plain torch ops.
 """
@@ -285,28 +287,55 @@ class GaussianDiffusion:
         """diffusion.py:245-250: KL(q(x_T|x_0) || N(0, I)) in bits per dimension."""
         from .functions import flat_mean, normal_kl
         B, T = len(x_0), self.timesteps
-        T_mean, _, T_logvar = self.q_mean_var(x_0=x_0, t=(T - 1) * torch.ones((B,), dtype=torch.int64))
+        T_mean, _, T_logvar = self.q_mean_var(x_0=x_0, t=(T - 1) * torch.ones((B,), dtype=torch.int64, device=x_0.device))
         zero = torch.zeros((), dtype=T_mean.dtype, device=T_mean.device)
         return flat_mean(normal_kl(T_mean, T_logvar, zero, zero)) / math.log(2.)
 
-    def calc_all_bpd(self, denoise_fn, x_0, clip_denoised=True):
+    # DDIM re-derives the tables on a sub-sequence; its calc_all_bpd keeps the generic formulas
+    _native_bpd = True
+
+    def calc_all_bpd(self, denoise_fn, x_0, clip_denoised=True, *, noise=None, use_graph=True):
         """diffusion.py:252-270.  Upstream unpacks ``B, T = x_0.shape, self.timesteps`` (B becomes the shape tuple and
         ``torch.empty([B, ])`` raises); this is the evident intent, B = batch size.
-        Returns (total_bpd [B], losses [B, T], prior_bpd [B], mses [B, T])."""
+        Returns (total_bpd [B], losses [B, T], prior_bpd [B], mses [B, T]), fp32 on the CPU as in the reference (:255-256).
+
+        Native path (a native UNet, eps-prediction, fixed variance, CUDA ``x_0``): every timestep is one engine launch
+        sequence (ddpm_bpd_step: q_sample in in_conv's loads, the UNet forward, the bound terms in the final conv's epilogue),
+        captured once into a CUDA graph and replayed T times, with no host synchronisation until the [B, T] results are copied
+        back.  Each step's noise is drawn like the generic loop's ``torch.randn_like(x_0)`` from the device's default
+        generator, so after ``torch.manual_seed(s)`` both paths see the same x_t sequence.  ``noise`` (optional,
+        [T, B, C, H, W]) replaces the draws: ``noise[ti]`` is used at step ti."""
+        model = self._fast_ok(denoise_fn)
+        if model is not None and x_0.is_cuda and self._native_bpd:
+            losses, mses = _native_bpd_loop(self, model, x_0.contiguous().float(), clip_denoised, noise, use_graph)
+        else:
+            losses, mses = self._generic_bpd_terms(denoise_fn, x_0, clip_denoised, noise)
+        prior_bpd = self._prior_bpd(x_0).cpu()
+        total_bpd = torch.sum(losses, dim=1) + prior_bpd
+        return total_bpd, losses, prior_bpd, mses
+
+    def _generic_bpd_terms(self, denoise_fn, x_0, clip_denoised, noise):
         from .functions import flat_mean
         B, T = len(x_0), self.timesteps
-        t = torch.empty([B, ], dtype=torch.int64)
-        losses = torch.zeros([B, T], dtype=torch.float32)
-        mses = torch.zeros([B, T], dtype=torch.float32)
+        t = torch.empty([B, ], dtype=torch.int64, device=x_0.device)
+        losses = torch.zeros([B, T], dtype=torch.float32, device=x_0.device)
+        mses = torch.zeros([B, T], dtype=torch.float32, device=x_0.device)
         for ti in range(T - 1, -1, -1):
             t.fill_(ti)
-            x_t = self.q_sample(x_0, t=t)
+            x_t = self.q_sample(x_0, t=t, noise=None if noise is None else noise[ti].to(x_0))
             loss, pred_x_0 = self._loss_term_bpd(denoise_fn, x_0, x_t=x_t, t=t, clip_denoised=clip_denoised, return_pred=True)
             losses[:, ti] = loss
             mses[:, ti] = flat_mean((pred_x_0 - x_0).pow(2))
-        prior_bpd = self._prior_bpd(x_0)
-        total_bpd = torch.sum(losses, dim=1) + prior_bpd
-        return total_bpd, losses, prior_bpd, mses
+        return losses.cpu(), mses.cpu()
+
+    def _bpd_rows(self):
+        """[T,9] fp32 rows {sqrt_ab, sqrt_1mab, sqrt_recip_ab, sqrt_recip_m1_ab, post_c1, post_c2, model_logvar, true_logvar,
+        t>0} of ddpm_bpd_setup; every entry goes through the same fp64 -> fp32 cast as ``_extract`` (diffusion.py:83)."""
+        f = lambda a: torch.as_tensor(a, dtype=torch.float32)
+        nz = (torch.arange(self.timesteps) > 0).float()
+        return torch.stack([f(self.sqrt_alphas_bar), f(self.sqrt_one_minus_alphas_bar), f(self.sqrt_recip_alphas_bar),
+                            f(self.sqrt_recip_m1_alphas_bar), f(self.posterior_mean_coef1), f(self.posterior_mean_coef2),
+                            f(self.fixed_model_logvar), f(self.posterior_logvar_clipped), nz], dim=1).contiguous()
 
     def _dev_tables(self, device):
         k = str(device)
@@ -488,3 +517,82 @@ def _native_sample_loop_on_device(diffusion, model, x, gen, rng, seed, use_graph
             draw()
             step()
     return x
+
+
+@torch.no_grad()
+def _native_bpd_loop(diffusion, model, x0, clip_denoised, noise, use_graph):
+    """The T timesteps of calc_all_bpd on the engine; returns CPU fp32 (losses [B, T], mses [B, T]).  Each step is
+    {noise draw, step-table fetch, q_sample + UNet forward, bound terms in the final conv's epilogue, fixed-order per-image
+    means}; with ``use_graph`` it is captured once per (shape, T, clip, plan) and replayed T times."""
+    L = _lib.lib()
+    dev = model.flat_params.device
+    if x0.device != dev:
+        raise RuntimeError(f"UNet lives on {dev} but x_0 is on {x0.device}")
+    B, _, H, W = x0.shape
+    T = diffusion.timesteps
+    if noise is not None and tuple(noise.shape) != (T,) + tuple(x0.shape):
+        raise ValueError(f"noise must be [T, B, C, H, W] = {[T] + list(x0.shape)}, got {list(noise.shape)}")
+    clip = int(bool(clip_denoised))
+    was_training = model.training
+    model.eval()
+    try:
+        with torch.cuda.device(dev):
+            # weights are re-packed at the head of the loop, as in the sampler loops: the reference EMA swaps values with
+            # `p.data.copy_` (utils/train.py:307-316), which no version counter sees
+            h = model.prepare(B, H, W, training=False, force_repack=True)
+            rows = diffusion._bpd_rows()
+            if model._bpd_T != T:                # the handle re-allocates its table: graphs holding the old one are stale
+                model._bpd_T, model._bpd_gen = T, model._bpd_gen + 1
+            _lib.check(L.ddpm_bpd_setup(h, T, rows.data_ptr()), "bpd_setup")
+            cur = torch.cuda.current_stream()
+            _lib.check(L.ddpm_bpd_reset(h, T - 1, C.c_void_p(cur.cuda_stream)), "bpd_reset")
+
+            def step(x, z, losses, mses):
+                _lib.check(L.ddpm_bpd_step(h, x.data_ptr(), z.data_ptr(), clip, losses.data_ptr(), mses.data_ptr(),
+                                           C.c_void_p(torch.cuda.current_stream().cuda_stream)), "bpd_step")
+
+            if noise is not None or not use_graph or T == 1:
+                losses = torch.empty((B, T), dtype=torch.float32, device=dev)
+                mses = torch.empty_like(losses)
+                if noise is not None:
+                    nz = noise.to(device=dev, dtype=torch.float32).contiguous()
+                    for ti in range(T - 1, -1, -1):
+                        step(x0, nz[ti], losses, mses)
+                else:
+                    z = torch.empty_like(x0)
+                    for _ in range(T):
+                        z.normal_()              # diffusion.py:93 torch.randn_like(x_0), same generator and order
+                        step(x0, z, losses, mses)
+                return losses.cpu(), mses.cpu()
+
+            # one cached graph per (shape, T, clip, plan): it owns persistent x_0 / noise / result buffers, so it serves every
+            # batch of that shape; the default generator advances its Philox offset on every replay exactly as an eager draw
+            key = ("bpd", tuple(x0.shape), T, clip, model._plan_epoch, model._bpd_gen)
+            ent = model._sampler_cache.get(key)
+            if ent is None:
+                if len(model._sampler_cache) >= 4:
+                    model._sampler_cache.clear()
+                ent = model._sampler_cache[key] = {"x": torch.empty_like(x0), "z": torch.empty_like(x0), "graph": None,
+                                                   "losses": torch.empty((B, T), dtype=torch.float32, device=dev),
+                                                   "mses": torch.empty((B, T), dtype=torch.float32, device=dev)}
+            xb, z, losses, mses = ent["x"], ent["z"], ent["losses"], ent["mses"]
+            xb.copy_(x0)
+            done = 0
+            if ent["graph"] is None:
+                z.normal_(); step(xb, z, losses, mses)      # first use: one eager step, then capture (capture does not execute)
+                done = 1
+                graph = torch.cuda.CUDAGraph()
+                side = torch.cuda.Stream()
+                side.wait_stream(cur)
+                with torch.cuda.stream(side):
+                    with torch.cuda.graph(graph, stream=side):
+                        z.normal_()
+                        step(xb, z, losses, mses)
+                cur.wait_stream(side)
+                ent["graph"] = graph
+            for _ in range(done, T):
+                ent["graph"].replay()
+            return losses.cpu(), mses.cpu()
+    finally:
+        if was_training:
+            model.train()

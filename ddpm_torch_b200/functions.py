@@ -1,7 +1,9 @@
 """Likelihood helpers of the reference's bits-per-dim path (ddpm_torch/functions.py:28-60, :99-101) — generic PyTorch
-formulas used by ``GaussianDiffusion._loss_term_bpd`` / ``calc_all_bpd`` / ``loss_type="kl"``.
-These paths are not on the accelerated hot path (no reference config uses them); they exist so that the host mirror
-covers the reference's public surface, and are parity-tested on CPU against goldens written by the unmodified reference."""
+formulas used by ``GaussianDiffusion._loss_term_bpd`` / ``calc_all_bpd`` / ``loss_type="kl"``, parity-tested on CPU against
+goldens written by the unmodified reference.
+``calc_all_bpd`` of a native UNet (eps-prediction, fixed variance, CUDA input) does not call them: the engine's bits/dim step
+(``bpd_elem`` in csrc/kernels_simt.cuh) repeats these operations in the same order in the epilogue of the UNet's final conv.
+``loss_type="kl"`` training stays on these formulas (it would need the backward of the bound)."""
 import math
 
 import torch

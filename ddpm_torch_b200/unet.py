@@ -91,7 +91,8 @@ class UNet(nn.Module):
         self._drop_calls = 0
         self._plan_epoch = 0
         self._sampler_cache = {}
-        self._acc = None                    # gradient-accumulation buffer (only exists when backward runs twice before a step)
+        self._bpd_T, self._bpd_gen = 0, 0    # chain length of the handle's bits/dim table and its allocation generation
+        self._acc = None                   # gradient-accumulation buffer (only exists when backward runs twice before a step)
         self._acc_pending = False
         self._bwd_since_zero = 0
         self.register_load_state_dict_post_hook(lambda module, incompatible: module.repack())

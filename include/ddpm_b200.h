@@ -155,6 +155,21 @@ int ddpm_sampler_step(ddpm_unet* h, float* x, const float* z, uint64_t seed, voi
 /* Same step, additionally writing the clipped x_0 prediction of diffusion.py:122,130 to pred_x0 f32[B,C,H,W] (NULL = skip):
  * GaussianDiffusion.p_sample_progressive (diffusion.py:176-198, p_sample_step(..., return_pred=True)). */
 int ddpm_sampler_step_pred(ddpm_unet* h, float* x, const float* z, uint64_t seed, float* pred_x0, void* stream);
+/* Log-likelihood in bits per dimension: one timestep of GaussianDiffusion.calc_all_bpd (diffusion.py:252-268) with its
+ * _loss_term_bpd (:203-215), eps-prediction and fixed variance.
+ * setup uploads the per-step rows coef[T][9] = {sqrt_ab, sqrt_1mab, sqrt_recip_ab, sqrt_recip_m1_ab, post_c1, post_c2,
+ * model_logvar, true_logvar, t>0} (HOST pointer; fp32 values cast from the fp64 tables as _extract does, diffusion.py:83).
+ * The table is owned by the handle, kept apart from the sampler's, and re-used when T is unchanged.
+ * reset(step) arms the device-side step counter (shared with the sampler); each step() call consumes one step ti (counter
+ * decrements): x_t = q_sample(x0, ti, noise) (diffusion.py:92-97) formed in in_conv's loads, eps = UNet(x_t, ti), then in the
+ * epilogue of the final conv (a tail kernel on plans whose out_conv is not on the tensor cores):
+ *   losses[b][ti] = mean_{c,y,x}(t > 0 ? KL(q(x_{t-1}|x_t,x_0) || p(x_{t-1}|x_t)) : -log p(x_0|x_1)) / ln 2
+ *   mses[b][ti]   = mean_{c,y,x}((pred_x0 - x0)^2),  pred_x0 clamped to [-1, 1] when clip_denoised != 0
+ * x0, noise f32[B,C,H,W]; losses, mses f32[B][T].  Per-block partial sums and a fixed-order finalise: no floating-point atomics.
+ * A step() is a fixed launch sequence with no host-side arguments that change -> capturable once, replayable T times. */
+int ddpm_bpd_setup(ddpm_unet* h, int T, const float* coef_host);
+int ddpm_bpd_reset(ddpm_unet* h, int first_step, void* stream);
+int ddpm_bpd_step(ddpm_unet* h, const float* x0, const float* noise, int clip_denoised, float* losses, float* mses, void* stream);
 /* Data-parallel training (train.py:110 DDP, utils/train.py:149-153): the backward pass finishes the flat gradient buffer in
  * contiguous CHUNKS, level group by level group, and records a CUDA event per chunk.  grad_chunks returns their number and
  * fills lo/hi (element offsets into the flat buffer, in completion order; together they tile it exactly); wait_grad_chunk makes
