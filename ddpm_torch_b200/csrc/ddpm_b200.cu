@@ -151,6 +151,8 @@ int ddpm_unet_backward(ddpm_unet* h, const float* d_eps, void* stream) {
 }
 int ddpm_train_forward(ddpm_unet* h, const float* x0, const int64_t* t, const float* noise, const float* tab_a, const float* tab_s,
                        float* losses, uint64_t dropout_seed, void* stream) {
+    // the loss compares eps with the noise element for element: both must have the image's channel count
+    if (h && h->e.cfg.in_channels != h->e.cfg.out_channels) return fail(-30, "ddpm_train_forward: eps prediction needs out_channels == in_channels");
     NEED_PLAN(h);
     UnetEngine& e = h->e;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -207,6 +209,8 @@ int ddpm_sampler_step(ddpm_unet* h, float* x, const float* z, uint64_t seed, voi
     return ddpm_sampler_step_pred(h, x, z, seed, nullptr, stream);
 }
 int ddpm_sampler_step_pred(ddpm_unet* h, float* x, const float* z, uint64_t seed, float* pred_x0, void* stream) {
+    // the step updates x_t in place from eps: both must have the image's channel count
+    if (h && h->e.cfg.in_channels != h->e.cfg.out_channels) return fail(-30, "ddpm_sampler_step: eps prediction needs out_channels == in_channels");
     NEED_PLAN(h);
     if (!h->d_coef) return fail(-33, "ddpm_sampler_setup has not been called");
     UnetEngine& e = h->e;

@@ -138,7 +138,8 @@ int ddpm_unet_forward(ddpm_unet* h, const float* x, const int64_t* t, float* eps
 /* Backward of the last forward: d_eps f32[B,Cout,H,W] -> flat grads (zeroed then written). x,t must be unchanged. */
 int ddpm_unet_backward(ddpm_unet* h, const float* d_eps, void* stream);
 /* Fused training forward (diffusion.py:217-243, mse/eps branch): x_t = q_sample(x0,t,noise) with the fp32 tables
- * tab_sqrt_ab / tab_sqrt_1mab [T]; eps = UNet(x_t,t); losses[b] = mean((noise-eps)^2). */
+ * tab_sqrt_ab / tab_sqrt_1mab [T]; eps = UNet(x_t,t); losses[b] = mean((noise-eps)^2).
+ * Needs out_channels == in_channels (fails before any launch otherwise), as do the sampler steps below. */
 int ddpm_train_forward(ddpm_unet* h, const float* x0, const int64_t* t, const float* noise, const float* tab_sqrt_ab,
                        const float* tab_sqrt_1mab, float* losses, uint64_t dropout_seed, void* stream);
 /* Backward of ddpm_train_forward given d(sum)/d(losses[b]) = gscale[b] (f32[B]). */
