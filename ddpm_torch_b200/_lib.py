@@ -50,6 +50,30 @@ class HaloDesc(C.Structure):
     ]
 
 
+class GnDesc(C.Structure):
+    _fields_ = [
+        ("route", C.c_int), ("B", C.c_int), ("HW", C.c_int), ("C0", C.c_int), ("C1", C.c_int),
+        ("x0", C.c_void_p), ("x1", C.c_void_p), ("gamma", C.c_void_p), ("beta", C.c_void_p),
+        ("silu", C.c_int), ("drop_p", C.c_float), ("seed", C.c_uint64), ("layer", C.c_uint32),
+        ("mask", C.c_void_p), ("qs0", C.c_void_p), ("qs1", C.c_void_p),
+        ("y", C.c_void_p), ("K", C.c_void_p), ("scratch", C.c_void_p),
+    ]
+
+
+class GnBwdDesc(C.Structure):
+    _fields_ = [
+        ("B", C.c_int), ("HW", C.c_int), ("C0", C.c_int), ("C1", C.c_int),
+        ("x0", C.c_void_p), ("x1", C.c_void_p), ("dy", C.c_void_p), ("K", C.c_void_p), ("gamma", C.c_void_p),
+        ("dgamma", C.c_void_p), ("dbeta", C.c_void_p),
+        ("dx0", C.c_void_p), ("dx1", C.c_void_p), ("acc0", C.c_int), ("acc1", C.c_int),
+        ("addend", C.c_void_p),
+        ("silu", C.c_int), ("drop_p", C.c_float), ("mask", C.c_void_p),
+        ("dn_inplace", C.c_int),
+        ("cs_per_img", C.c_void_p), ("cs_ld", C.c_int), ("cs_total", C.c_void_p), ("cs_total2", C.c_void_p),
+        ("scratch", C.c_void_p),
+    ]
+
+
 class UnetCfg(C.Structure):
     _fields_ = [("in_channels", C.c_int), ("hid_channels", C.c_int), ("out_channels", C.c_int),
                 ("levels", C.c_int), ("ch_mult", C.c_int * 8), ("num_res_blocks", C.c_int), ("attn", C.c_int * 8),
@@ -83,6 +107,10 @@ def lib():
             "ddpm_conv_halo_run": ([C.POINTER(HaloDesc), vp], i32),
             "ddpm_attn_fused_run": ([vp, vp, vp, i32, i32, i32, vp], i32),
             "ddpm_attn_fused_bwd_run": ([vp, vp, vp, vp, vp, i32, i32, i32, vp], i32),
+            "ddpm_gn_scratch_bytes": ([i32, i32], i64),
+            "ddpm_groupnorm_fwd_run": ([C.POINTER(GnDesc), vp], i32),
+            "ddpm_groupnorm_bwd_run": ([C.POINTER(GnBwdDesc), vp], i32),
+            "ddpm_colsum_run": ([vp, vp, i32, vp, vp, i32, i32, i32, i32, vp], i32),
             "ddpm_unet_create": ([C.POINTER(UnetCfg), C.POINTER(vp)], i32),
             "ddpm_unet_destroy": ([vp], None),
             "ddpm_unet_num_params": ([vp], i32),
@@ -120,6 +148,7 @@ def lib():
 
 
 EXPORTS = ["ddpm_last_error", "ddpm_runtime_check", "ddpm_device_error_flag", "ddpm_gemm_run", "ddpm_conv_halo_run", "ddpm_attn_fused_run", "ddpm_attn_fused_bwd_run",
+           "ddpm_gn_scratch_bytes", "ddpm_groupnorm_fwd_run", "ddpm_groupnorm_bwd_run", "ddpm_colsum_run",
            "ddpm_unet_create", "ddpm_unet_destroy", "ddpm_unet_num_params", "ddpm_unet_param_info",
            "ddpm_unet_flat_elems", "ddpm_unet_workspace_bytes", "ddpm_unet_plan", "ddpm_unet_repack",
            "ddpm_unet_forward", "ddpm_unet_backward", "ddpm_train_forward", "ddpm_train_backward",

@@ -71,6 +71,105 @@ int ddpm_attn_fused_bwd_run(const void* qkv, const void* d_out, const void* prob
     return launch_attn_bwd(g, static_cast<cudaStream_t>(stream));
 }
 
+// ------------------------------------------------------------------------------------------------ GroupNorm / column sums
+// scratch layout.  forward: stats f64 [B][64] | tickets i32 [B].  backward: cs f32 [B][2][C] | tickets i32 [B] | PQ f32 [B][2][C]
+static size_t gn_align(size_t n) { return (n + 255) & ~size_t(255); }
+static size_t gn_fwd_scratch(int B) { return gn_align((size_t)B * 64 * 8) + gn_align((size_t)B * 4); }
+static size_t gn_bwd_scratch(int B, int C) { return 2 * gn_align((size_t)B * 2 * C * 4) + gn_align((size_t)B * 4); }
+static bool misaligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; }
+static int gn_check_src(const char* fn, int B, int HW, int C0, int C1, const void* x0, const void* x1) {
+    if (B < 1 || HW < 1) return fail(-42, "%s: need B >= 1 and HW >= 1", fn);
+    if (C0 < 8 || C0 % 8 || C1 < 0 || C1 % 8) return fail(-42, "%s: C0 and C1 must be multiples of 8 (C0 > 0, C1 >= 0)", fn);
+    const int C = C0 + C1;
+    if (C % 32) return fail(-42, "%s: C = C0 + C1 = %d must be a multiple of 32 (32 groups)", fn, C);
+    if (C > kGnMaxC) return fail(-42, "%s: C = %d exceeds the supported maximum of %d channels", fn, C, kGnMaxC);
+    if (!x0 || (C1 && !x1)) return fail(-42, "%s: null source", fn);
+    if (misaligned16(x0) || misaligned16(x1)) return fail(-42, "%s: sources must be 16-byte aligned", fn);
+    return 0;
+}
+
+long long ddpm_gn_scratch_bytes(int B, int C) {
+    if (B < 1 || C < 1) return fail(-42, "ddpm_gn_scratch_bytes: need B >= 1 and C >= 1");
+    const size_t f = gn_fwd_scratch(B), b = gn_bwd_scratch(B, C);
+    return (long long)(f > b ? f : b);
+}
+
+int ddpm_groupnorm_fwd_run(const ddpm_gn_desc* d, void* stream) {
+    const char* fn = "ddpm_groupnorm_fwd_run";
+    if (!d) return fail(-42, "%s: null descriptor", fn);
+    int rc = gn_check_src(fn, d->B, d->HW, d->C0, d->C1, d->x0, d->x1);
+    if (rc) return rc;
+    const int C = d->C0 + d->C1, B = d->B, r = d->route;
+    if (r < 1 || r > 4) return fail(-42, "%s: route must be 1 (stats + apply), 2 (small), 3 (quad statistics) or 4 (prep)", fn);
+    if (r == 2 && d->HW > 64) return fail(-42, "%s: route 2 needs HW <= 64 (got %d)", fn, d->HW);
+    if (r >= 3 && C % 128) return fail(-42, "%s: routes 3 and 4 need C %% 128 == 0 (got %d)", fn, C);
+    if (r >= 3 && (!d->qs0 || (d->C1 && !d->qs1))) return fail(-42, "%s: routes 3 and 4 need the quad statistics qs0 / qs1", fn);
+    if (!d->gamma || !d->beta || !d->K || (r != 4 && !d->y) || (r == 1 && !d->scratch)) return fail(-42, "%s: null buffer", fn);
+    if (misaligned16(d->gamma) || misaligned16(d->beta) || misaligned16(d->K) || misaligned16(d->y))
+        return fail(-42, "%s: gamma, beta, K and y must be 16-byte aligned", fn);
+    if (!(d->drop_p >= 0.f && d->drop_p < 1.f)) return fail(-42, "%s: drop_p must be in [0, 1)", fn);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    GnApply a; memset(&a, 0, sizeof a);
+    a.s.x0 = static_cast<const bf16*>(d->x0); a.s.x1 = static_cast<const bf16*>(d->x1); a.s.C0 = d->C0; a.s.C1 = d->C1;
+    a.K = d->K; a.y = static_cast<bf16*>(d->y); a.HW = d->HW; a.silu = d->silu ? 1 : 0; a.drop_p = d->drop_p; a.layer = d->layer; a.mask = d->mask;
+    gn_arm_dropout(a.drop_p, a.seed, (unsigned long long)d->seed);
+    a.gamma = d->gamma; a.beta = d->beta; a.eps = 1e-6f; a.Kout = d->K;
+    if (r == 1) {
+        a.gamma = nullptr; a.beta = nullptr; a.Kout = nullptr;        // the apply pass reads the K the statistics pass finalised
+        uint8_t* s = static_cast<uint8_t*>(d->scratch);
+        GnFin fin; fin.gamma = d->gamma; fin.beta = d->beta; fin.K = d->K; fin.eps = 1e-6f;
+        fin.ticket = reinterpret_cast<int*>(s + gn_align((size_t)B * 64 * 8));
+        if ((rc = launch_gn_stats(a.s, reinterpret_cast<double*>(s), B, d->HW, fin, st))) return fail(-20, "%s: %s", fn, cudaGetErrorString((cudaError_t)rc));
+        rc = launch_gn_apply(a, B, st);
+    } else if (r == 2) {
+        rc = launch_gn_small(a, B, st);
+    } else {
+        a.qs0 = d->qs0; a.qs1 = d->C1 ? d->qs1 : nullptr;
+        rc = r == 3 ? launch_gn_apply(a, B, st) : launch_gn_prep(a, B, st);
+    }
+    return rc ? fail(-20, "%s: %s", fn, cudaGetErrorString((cudaError_t)rc)) : 0;
+}
+
+int ddpm_groupnorm_bwd_run(const ddpm_gn_bwd_desc* d, void* stream) {
+    const char* fn = "ddpm_groupnorm_bwd_run";
+    if (!d) return fail(-42, "%s: null descriptor", fn);
+    int rc = gn_check_src(fn, d->B, d->HW, d->C0, d->C1, d->x0, d->x1);
+    if (rc) return rc;
+    const int C = d->C0 + d->C1, B = d->B;
+    if (!d->dy || !d->K || !d->gamma || !d->dgamma || !d->dbeta || !d->dx0 || (d->C1 && !d->dx1) || !d->scratch)
+        return fail(-42, "%s: null buffer", fn);
+    if (misaligned16(d->dy) || misaligned16(d->K) || misaligned16(d->dx0) || misaligned16(d->dx1) || misaligned16(d->addend))
+        return fail(-42, "%s: dy, K, dx0, dx1 and addend must be 16-byte aligned", fn);
+    if (!(d->drop_p >= 0.f && d->drop_p < 1.f)) return fail(-42, "%s: drop_p must be in [0, 1)", fn);
+    if (d->drop_p > 0.f && !d->mask) return fail(-42, "%s: drop_p > 0 needs the forward's dropout mask", fn);
+    if (d->cs_per_img && d->cs_ld < C) return fail(-42, "%s: cs_ld must be >= C", fn);
+    GnBwd a; memset(&a, 0, sizeof a);
+    a.s.x0 = static_cast<const bf16*>(d->x0); a.s.x1 = static_cast<const bf16*>(d->x1); a.s.C0 = d->C0; a.s.C1 = d->C1;
+    a.dy = static_cast<const bf16*>(d->dy); a.K = d->K; a.gamma = d->gamma;
+    uint8_t* s = static_cast<uint8_t*>(d->scratch);
+    const size_t cs_bytes = gn_align((size_t)B * 2 * C * 4);
+    a.cs = reinterpret_cast<float*>(s); a.ticket = reinterpret_cast<int*>(s + cs_bytes);
+    a.PQ = reinterpret_cast<float*>(s + cs_bytes + gn_align((size_t)B * 4));
+    a.dgamma = d->dgamma; a.dbeta = d->dbeta;
+    a.dx0 = static_cast<bf16*>(d->dx0); a.dx1 = d->C1 ? static_cast<bf16*>(d->dx1) : nullptr; a.acc0 = d->acc0 ? 1 : 0; a.acc1 = d->acc1 ? 1 : 0;
+    a.addend = static_cast<const bf16*>(d->addend); a.B = B; a.HW = d->HW; a.silu = d->silu ? 1 : 0;
+    a.drop_p = d->drop_p; a.mask = d->mask; a.dn_inplace = d->dn_inplace ? 1 : 0;
+    rc = launch_gn_bwd(a, d->cs_per_img, d->cs_ld, d->cs_total, d->cs_total2, static_cast<cudaStream_t>(stream));
+    return rc ? fail(-20, "%s: %s", fn, cudaGetErrorString((cudaError_t)rc)) : 0;
+}
+
+int ddpm_colsum_run(const void* dy, float* per_img, int ld, float* total, float* total2, int B, int HW, int C, int C_valid, void* stream) {
+    const char* fn = "ddpm_colsum_run";
+    if (!dy) return fail(-42, "%s: null dy", fn);
+    if (misaligned16(dy)) return fail(-42, "%s: dy must be 16-byte aligned", fn);
+    if (B < 1 || HW < 1) return fail(-42, "%s: need B >= 1 and HW >= 1", fn);
+    if (C < 8 || C % 8) return fail(-42, "%s: C must be a positive multiple of 8", fn);
+    if (C_valid < 1 || C_valid > C) return fail(-42, "%s: need 1 <= C_valid <= C", fn);
+    if (per_img && ld < C_valid) return fail(-42, "%s: ld must be >= C_valid", fn);
+    const int rc = launch_colsum(static_cast<const bf16*>(dy), per_img, ld, total, total2, B, HW, C, C_valid, static_cast<cudaStream_t>(stream));
+    return rc ? fail(-20, "%s: %s", fn, cudaGetErrorString((cudaError_t)rc)) : 0;
+}
+
 // ------------------------------------------------------------------------------------------------ UNet engine
 int ddpm_unet_create(const ddpm_unet_cfg* cfg, ddpm_unet** out) {
     if (!cfg || !out) return fail(-30, "null argument");

@@ -1092,34 +1092,40 @@ __global__ void __launch_bounds__(256) k_chansum_nchw(const float* __restrict__ 
 }
 // ============================================================================ column sums: per image and total
 // dy [B][HW][C] bf16 -> per_img[b][ld] (+=, fp32 atomics, optional) and total[c] (+=)
+// grid (pixel blocks, B, channel slices): blockIdx.z covers channels [z*cs, z*cs + cs) of a C wider than one block's 256 octets
 __global__ void __launch_bounds__(256) k_colsum(const bf16* __restrict__ dy, float* per_img, int ld, float* total, float* total2,
-                                               int HW, int C, int C_valid, int pix_per_block) {
+                                               int HW, int C, int C_valid, int pix_per_block, int cs) {
     pdl_entry();
-    // blockDim.x = (256/oct)*oct: one channel octet per thread; partials are merged in shared memory so that each block
-    // issues ONE atomic per channel (the first version issued one per thread and spent 14 ms/step in contention)
-    extern __shared__ float sh[];                 // [C]
+    // blockDim.x = (256/oct)*oct with oct = cs/8: one channel octet per thread; partials are merged in shared memory so that each
+    // block issues ONE atomic per channel (the first version issued one per thread and spent 14 ms/step in contention)
+    extern __shared__ float sh[];                 // [cs]
     const int b = blockIdx.y;
     const int p0 = blockIdx.x * pix_per_block;
     int p1 = p0 + pix_per_block; if (p1 > HW) p1 = HW;
-    const int oct = C >> 3;
-    for (int i = threadIdx.x; i < C; i += blockDim.x) sh[i] = 0.f;
+    const int c0 = blockIdx.z * cs;
+    const int w = C - c0 < cs ? C - c0 : cs;      // width of this slice (the last one may be narrower)
+    const int oct = cs >> 3;
+    for (int i = threadIdx.x; i < cs; i += blockDim.x) sh[i] = 0.f;
     __syncthreads();
     const int o = threadIdx.x % oct, lp = threadIdx.x / oct, pstep = blockDim.x / oct;
     float s[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    for (int p = p0 + lp; p < p1; p += pstep) {
-        float f[8];
-        unpack8(__ldg(reinterpret_cast<const uint4*>(dy + ((long long)b * HW + p) * C + o * 8)), f);
+    if (o * 8 < w) {
+        for (int p = p0 + lp; p < p1; p += pstep) {
+            float f[8];
+            unpack8(__ldg(reinterpret_cast<const uint4*>(dy + ((long long)b * HW + p) * C + c0 + o * 8)), f);
 #pragma unroll
-        for (int e = 0; e < 8; ++e) s[e] += f[e];
+            for (int e = 0; e < 8; ++e) s[e] += f[e];
+        }
     }
 #pragma unroll
     for (int e = 0; e < 8; ++e) atomicAdd(&sh[o * 8 + e], s[e]);
     __syncthreads();
-    for (int i = threadIdx.x; i < C_valid; i += blockDim.x) {
+    const int nv = C_valid - c0 < w ? C_valid - c0 : w;
+    for (int i = threadIdx.x; i < nv; i += blockDim.x) {
         const float v = sh[i];
-        if (per_img) atomicAdd(per_img + (long long)b * ld + i, v);
-        if (total) atomicAdd(total + i, v);
-        if (total2) atomicAdd(total2 + i, v);
+        if (per_img) atomicAdd(per_img + (long long)b * ld + c0 + i, v);
+        if (total) atomicAdd(total + c0 + i, v);
+        if (total2) atomicAdd(total2 + c0 + i, v);
     }
 }
 

@@ -34,6 +34,67 @@ struct GnSaved { Src in; float* K; const float* gamma; const float* beta; float*
 static inline int grid_for(long long n, int threads = 256) { long long g = (n + threads - 1) / threads; if (g > kPlanSms * 16) g = kPlanSms * 16; if (g < 1) g = 1; return (int)g; }
 static inline int oct_threads(int C) { const int oct = C / 8; return oct <= 256 ? (256 / oct) * oct : 0; }
 
+// ------------------------------------------------------------------ GroupNorm / column-sum launches
+// Shared by the engine's plans and the GroupNorm operators of the C ABI, so that both launch the same geometry.
+// The GroupNorm kernels give every thread one channel octet of the concat for its whole pixel loop: at most 256 octets.
+constexpr int kGnMaxC = 2048;
+// blocks over the pixels of one image: keep the whole launch within one wave of (kPlanSms x occ) CTAs
+static inline void gn_grid(int Bn, int HW, int occ, int& nblk, int& ppb) {
+    nblk = (kPlanSms * occ) / Bn; if (nblk > HW / 16) nblk = HW / 16; if (nblk < 1) nblk = 1;
+    ppb = (HW + nblk - 1) / nblk; nblk = (HW + ppb - 1) / ppb;
+}
+// Grid granularity (DDPM_GN_STATS_OCC / _APPLY_OCC / _BWD_OCC override it): blocks per image = kPlanSms*occ/B with occ 4 -
+// finer grids pay more per-block prologue / atomics than the wave-quantisation they would save.
+static inline int gn_occ(const char* env) { const char* v = getenv(env); return v ? atoi(v) : 4; }
+// k_gn_stats: fp64 {sum, sumsq} per (image, group) into the zeroed stats[B][64]; the last block of an image writes fin.K
+static inline int launch_gn_stats(const GnSrc& s, double* stats, int Bn, int HW, const GnFin& fin, cudaStream_t st) {
+    static const int occ = gn_occ("DDPM_GN_STATS_OCC");
+    int nblk, ppb; gn_grid(Bn, HW, occ, nblk, ppb);
+    launch_k(k_gn_stats, dim3(nblk, Bn), oct_threads(s.C0 + s.C1), 0, st, s, stats, HW, ppb, fin);
+    return (int)cudaGetLastError();
+}
+// k_gn_apply: y = act(x*sc + sh) [* dropout], sc/sh from a.K, or from the producers' quad statistics when a.qs0 is set
+static inline int launch_gn_apply(const GnApply& a, int Bn, cudaStream_t st) {
+    static const int occ = gn_occ("DDPM_GN_APPLY_OCC");
+    int nblk, ppb; gn_grid(Bn, a.HW, occ, nblk, ppb);
+    launch_k(k_gn_apply, dim3(nblk, Bn), oct_threads(a.s.C0 + a.s.C1), 0, st, a, ppb);
+    return (int)cudaGetLastError();
+}
+// k_gn_small: statistics + apply in one launch, one block per image (HW <= 64)
+static inline int launch_gn_small(const GnApply& a, int Bn, cudaStream_t st) {
+    launch_k(k_gn_small, Bn, oct_threads(a.s.C0 + a.s.C1), 0, st, a);
+    return (int)cudaGetLastError();
+}
+// k_gn_prep: a.Kout from the producers' quad statistics, no pass over the tensor
+static inline int launch_gn_prep(const GnApply& a, int Bn, cudaStream_t st) {
+    const int C = a.s.C0 + a.s.C1;
+    launch_k(k_gn_prep, Bn, C < 256 ? C : 256, 0, st, a);
+    return (int)cudaGetLastError();
+}
+// dropout is armed per call by a non-zero seed
+static inline void gn_arm_dropout(float& drop_p, unsigned long long& seed, unsigned long long run_seed) { seed = run_seed; if (!seed) drop_p = 0.f; }
+// k_gn_bwd_reduce + k_gn_bwd_apply; the apply pass also accumulates the column sums of dx when any of the cs pointers is set
+static inline int launch_gn_bwd(const GnBwd& a0, float* cs_per_img, int cs_ld, float* cs_total, float* cs_total2, cudaStream_t st) {
+    static const int occ = gn_occ("DDPM_GN_BWD_OCC");
+    GnBwd a = a0;
+    int nblk; gn_grid(a.B, a.HW, occ, nblk, a.pix_per_block);
+    const int C = a.s.C0 + a.s.C1, thr = oct_threads(C);
+    const dim3 g(nblk, a.B);
+    launch_k(k_gn_bwd_reduce, g, thr, (size_t)2 * C * 4, st, a);
+    if (cs_per_img || cs_total || cs_total2) launch_k(k_gn_bwd_apply<true>, g, thr, (size_t)C * 4, st, a, cs_per_img, cs_ld, cs_total, cs_total2);
+    else                                     launch_k(k_gn_bwd_apply<false>, g, thr, 0, st, a, cs_per_img, cs_ld, cs_total, cs_total2);
+    return (int)cudaGetLastError();
+}
+// k_colsum over dy [B][HW][C]: column sums of the first C_valid channels; C above kGnMaxC runs as kGnMaxC-wide slices in grid z
+static inline int launch_colsum(const bf16* dy, float* per_img, int ld, float* total, float* total2, int Bn, int HW, int C, int C_valid,
+                                cudaStream_t st) {
+    const int cs = C < kGnMaxC ? C : kGnMaxC, nz = (C + cs - 1) / cs;
+    int nblk = (592 + Bn - 1) / Bn; if (nblk > HW / 8) nblk = HW / 8; if (nblk < 1) nblk = 1;
+    const int ppb = (HW + nblk - 1) / nblk; nblk = (HW + ppb - 1) / ppb;
+    launch_k(k_colsum, dim3(nblk, Bn, nz), oct_threads(cs), (size_t)cs * 4, st, dy, per_img, ld, total, total2, HW, C, C_valid, ppb, cs);
+    return (int)cudaGetLastError();
+}
+
 struct UnetEngine {
     ddpm_unet_cfg cfg;
     std::vector<ParamInfo> params;
@@ -186,12 +247,12 @@ struct UnetEngine {
     }
     float* gn_prep_xf(std::vector<Op>& L, const std::string& name, const Src& in, const std::string& pname) {
         const int C = in.C(), Bn = in.t0.B, HW = in.t0.H * in.t0.W;
+        gn_check(name, C);
         float* K = at<float>(alloc((size_t)Bn * 4 * C * 4));
         GnApply a; memset(&a, 0, sizeof a);
         a.s = gsrc(in); a.HW = HW; a.qs0 = at<double>((size_t)in.t0.qs); a.qs1 = nullptr;
         a.gamma = PP(pname + ".weight"); a.beta = PP(pname + ".bias"); a.eps = 1e-6f; a.Kout = K;
-        const int thr = C < 256 ? C : 256;
-        push(L, name + ".prep", 0, [a, Bn, thr](cudaStream_t st) { launch_k(k_gn_prep, Bn, thr, 0, st, a); return (int)cudaGetLastError(); });
+        push(L, name + ".prep", 0, [a, Bn](cudaStream_t st) { return launch_gn_prep(a, Bn, st); });
         return K;
     }
     // epilogue fusion of a conv: fills `gn` and returns the workspace offset of the quad statistics (-1: none)
@@ -403,60 +464,43 @@ struct UnetEngine {
     size_t zero_fwd(size_t bytes) { const size_t o = zf_cursor; zf_cursor += (bytes + 255) & ~size_t(255); return zero_fwd_off + o; }
     size_t zero_bwd(size_t bytes) { const size_t o = zb_cursor; zb_cursor += (bytes + 255) & ~size_t(255); return zero_bwd_off + o; }
 
-    // blocks over the pixels of one image: keep the whole launch within one wave of (kPlanSms x occ) CTAs
-    static void gn_grid(int Bn, int HW, int occ, int& nblk, int& ppb) {
-        nblk = (kPlanSms * occ) / Bn; if (nblk > HW / 16) nblk = HW / 16; if (nblk < 1) nblk = 1;
-        ppb = (HW + nblk - 1) / nblk; nblk = (HW + ppb - 1) / ppb;
+    // a GroupNorm over more than kGnMaxC concat channels has no launch geometry: refuse the plan, naming the first such layer
+    void gn_check(const std::string& name, int C) {
+        if (C > kGnMaxC && !plan_error)
+            plan_error = fail(-30, "GroupNorm '%s' has %d channels; the GroupNorm kernels support at most %d", name.c_str(), C, kGnMaxC);
     }
     GnSaved gn_fwd(std::vector<Op>& L, const std::string& name, const Src& in, const std::string& pname, const T4& out, int silu, float drop_p) {
         const int C = in.C(), Bn = in.t0.B, HW = in.t0.H * in.t0.W;
-        GnSaved sv; sv.in = in; sv.silu = silu; sv.drop_p = drop_p; sv.layer = ++layer_counter;   // dropout is armed per call by a non-zero seed
+        gn_check(name, C);
+        GnSaved sv; sv.in = in; sv.silu = silu; sv.drop_p = drop_p; sv.layer = ++layer_counter;
         sv.gamma = PP(pname + ".weight"); sv.beta = PP(pname + ".bias"); sv.dgamma = GP(pname + ".weight"); sv.dbeta = GP(pname + ".bias");
         double* stats = at<double>(zero_fwd((size_t)Bn * 64 * 8));
         sv.K = at<float>(alloc((size_t)Bn * 4 * C * 4));
         const GnSrc gs = gsrc(in);
-        const int thr = oct_threads(C);
         float* K = sv.K; const float* ga = sv.gamma; const float* be = sv.beta;
         sv.mask = (drop_p > 0.f && train) ? at<unsigned char>(alloc((size_t)Bn * HW * (C / 8))) : nullptr;
+        GnApply a; memset(&a, 0, sizeof a);
+        a.s = gs; a.K = K; a.y = bp(out); a.HW = HW; a.silu = silu; a.drop_p = sv.drop_p; a.seed = 0; a.layer = sv.layer; a.mask = sv.mask;
+        UnetEngine* self = this;
         // statistics delivered by the producers' epilogues (conv_gn_epi): one launch, no pass over the tensor for the stats
         const bool have_qs = in.t0.qs >= 0 && (!in.two || in.t1.qs >= 0) && (C % 128) == 0;
         if (have_qs) {
-            static const int ap_occ = getenv("DDPM_GN_APPLY_OCC") ? atoi(getenv("DDPM_GN_APPLY_OCC")) : 4;
-            GnApply a; memset(&a, 0, sizeof a);
-            a.s = gs; a.K = K; a.y = bp(out); a.HW = HW; a.silu = silu; a.drop_p = sv.drop_p; a.seed = 0; a.layer = sv.layer; a.mask = sv.mask;
             a.qs0 = at<double>((size_t)in.t0.qs); a.qs1 = in.two ? at<double>((size_t)in.t1.qs) : nullptr;
             a.gamma = ga; a.beta = be; a.eps = 1e-6f; a.Kout = K;
-            int nb2, ppb2; gn_grid(Bn, HW, ap_occ, nb2, ppb2);
-            const dim3 g2(nb2, Bn);
-            UnetEngine* self = this;
-            push(L, name + ".apply[qs]", 0, [a, g2, thr, ppb2, self](cudaStream_t st) { GnApply aa = a; aa.seed = self->drop_seed; if (!aa.seed) aa.drop_p = 0.f;
-                launch_k(k_gn_apply, g2, thr, 0, st, aa, ppb2); return (int)cudaGetLastError(); });
+            push(L, name + ".apply[qs]", 0, [a, Bn, self](cudaStream_t st) { GnApply aa = a; gn_arm_dropout(aa.drop_p, aa.seed, self->drop_seed);
+                return launch_gn_apply(aa, Bn, st); });
             return sv;
         }
         if (HW <= 64 && !getenv("DDPM_NO_GN_EPI")) {       // tiny maps: statistics + apply in ONE launch, one block per image
-            GnApply a; memset(&a, 0, sizeof a);
-            a.s = gs; a.K = K; a.y = bp(out); a.HW = HW; a.silu = silu; a.drop_p = sv.drop_p; a.seed = 0; a.layer = sv.layer; a.mask = sv.mask;
             a.gamma = ga; a.beta = be; a.eps = 1e-6f; a.Kout = K;
-            UnetEngine* self = this;
-            push(L, name + ".small", 0, [a, Bn, thr, self](cudaStream_t st) { GnApply aa = a; aa.seed = self->drop_seed; if (!aa.seed) aa.drop_p = 0.f;
-                launch_k(k_gn_small, Bn, thr, 0, st, aa); return (int)cudaGetLastError(); });
+            push(L, name + ".small", 0, [a, Bn, self](cudaStream_t st) { GnApply aa = a; gn_arm_dropout(aa.drop_p, aa.seed, self->drop_seed);
+                return launch_gn_small(aa, Bn, st); });
             return sv;
         }
-        static const int st_occ = getenv("DDPM_GN_STATS_OCC") ? atoi(getenv("DDPM_GN_STATS_OCC")) : 4;
-        static const int ap_occ = getenv("DDPM_GN_APPLY_OCC") ? atoi(getenv("DDPM_GN_APPLY_OCC")) : 4;
-        int nblk, ppb; gn_grid(Bn, HW, st_occ, nblk, ppb);
-        const dim3 g1(nblk, Bn);
         GnFin fin; fin.gamma = ga; fin.beta = be; fin.K = K; fin.eps = 1e-6f; fin.ticket = at<int>(zero_fwd((size_t)Bn * 4));
-        push(L, name + ".stats", 0, [=](cudaStream_t st) {
-            launch_k(k_gn_stats, g1, thr, 0, st, gs, stats, HW, ppb, fin);
-            return (int)cudaGetLastError(); });
-        GnApply a; memset(&a, 0, sizeof a);
-        a.s = gs; a.K = K; a.y = bp(out); a.HW = HW; a.silu = silu; a.drop_p = sv.drop_p; a.seed = 0; a.layer = sv.layer; a.mask = sv.mask;
-        int nb2, ppb2; gn_grid(Bn, HW, ap_occ, nb2, ppb2);
-        const dim3 g2(nb2, Bn);
-        UnetEngine* self = this;
-        push(L, name + ".apply", 0, [a, g2, thr, ppb2, self](cudaStream_t st) { GnApply aa = a; aa.seed = self->drop_seed; if (!aa.seed) aa.drop_p = 0.f;
-            launch_k(k_gn_apply, g2, thr, 0, st, aa, ppb2); return (int)cudaGetLastError(); });
+        push(L, name + ".stats", 0, [=](cudaStream_t st) { return launch_gn_stats(gs, stats, Bn, HW, fin, st); });
+        push(L, name + ".apply", 0, [a, Bn, self](cudaStream_t st) { GnApply aa = a; gn_arm_dropout(aa.drop_p, aa.seed, self->drop_seed);
+            return launch_gn_apply(aa, Bn, st); });
         return sv;
     }
     // dx(in) (=|+=) gn_bwd(dy) + addend ; dgamma/dbeta accumulate into the flat grads
@@ -475,31 +519,15 @@ struct UnetEngine {
         a.ticket = at<int>(zero_bwd((size_t)Bn * 4));
         static const bool no_dn = getenv("DDPM_GN_NO_DN") != nullptr;
         a.dn_inplace = (sv.silu && !no_dn) ? 1 : 0;
-        const int thr = oct_threads(C);
-        // Grid granularity (DDPM_GN_BWD_OCC / _STATS_OCC / _APPLY_OCC override it): blocks per image = kPlanSms*occ/B with occ 4 -
-        // finer grids pay more per-block prologue / atomics than the wave-quantisation they would save.
-        static const int gn_bwd_occ = getenv("DDPM_GN_BWD_OCC") ? atoi(getenv("DDPM_GN_BWD_OCC")) : 4;
-        int nblk, ppb; gn_grid(Bn, HW, gn_bwd_occ, nblk, ppb);
-        a.pix_per_block = ppb;
-        const dim3 g1(nblk, Bn);
-        const size_t shm = (size_t)2 * C * 4;
-        const size_t shm2 = (cs_per_img || cs_total || cs_total2) ? (size_t)C * 4 : 0;
         UnetEngine* self = this;
         push(bwd_ops, name + ".gn_bwd", 0, [=](cudaStream_t st) {
-            GnBwd aa = a; aa.seed = self->drop_seed; if (!aa.seed) aa.drop_p = 0.f;
-            launch_k(k_gn_bwd_reduce, g1, thr, shm, st, aa);
-            if (shm2) launch_k(k_gn_bwd_apply<true>, g1, thr, shm2, st, aa, cs_per_img, cs_ld, cs_total, cs_total2);
-            else      launch_k(k_gn_bwd_apply<false>, g1, thr, 0, st, aa, cs_per_img, cs_ld, cs_total, cs_total2);
-            return (int)cudaGetLastError(); }, 2);
+            GnBwd aa = a; gn_arm_dropout(aa.drop_p, aa.seed, self->drop_seed);
+            return launch_gn_bwd(aa, cs_per_img, cs_ld, cs_total, cs_total2, st); }, 2);
     }
     void colsum_op(const std::string& name, const T4& dy, float* per_img, int ld, float* total, float* total2, int C_valid) {
         const int HW = dy.H * dy.W, C = dy.C, Bn = dy.B;
-        const int thr = oct_threads(C);
-        int nblk = (592 + Bn - 1) / Bn; if (nblk > HW / 8) nblk = HW / 8; if (nblk < 1) nblk = 1;
-        const int ppb = (HW + nblk - 1) / nblk; nblk = (HW + ppb - 1) / ppb;
-        const dim3 g(nblk, Bn); const bf16* p = bp(dy);
-        const size_t shm = (size_t)C * 4;
-        push(bwd_ops, name + ".colsum", 0, [=](cudaStream_t st) { launch_k(k_colsum, g, thr, shm, st, p, per_img, ld, total, total2, HW, C, C_valid, ppb); return (int)cudaGetLastError(); }, 1, /*side=*/true);
+        const bf16* p = bp(dy);
+        push(bwd_ops, name + ".colsum", 0, [=](cudaStream_t st) { return launch_colsum(p, per_img, ld, total, total2, Bn, HW, C, C_valid, st); }, 1, /*side=*/true);
     }
 
     // ------------------------------------------------------------------ packed weights (table-driven: one launch re-packs everything)

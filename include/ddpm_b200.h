@@ -104,6 +104,58 @@ int ddpm_attn_fused_run(const void* qkv, void* out, void* probs, int NB, int T, 
 int ddpm_attn_fused_bwd_run(const void* qkv, const void* d_out, const void* probs, void* d_scores, void* d_qkv, int NB, int T, int C, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Low-level operators: GroupNorm(32, C, eps=1e-6) [+ SiLU] [+ dropout] (unet.py:18-20,83-84) and the bias column sums, with the
+ * launch geometry the UNet engine's plans use (used by the parity tests of the engine itself).
+ * Input = channel concat of two NHWC bf16 sources x0 [B][HW][C0] and x1 [B][HW][C1] (C1 = 0: one source).  C0 and C1 are
+ * multiples of 8, C = C0 + C1 is a multiple of 32 and at most 2048.  Arguments are checked before any device work.
+ * scratch: caller-owned device area of ddpm_gn_scratch_bytes(B, C) bytes, zeroed by the caller before every call.
+ *
+ * Forward routes (the engine picks one per norm from the shape):
+ *  1  k_gn_stats + k_gn_apply (fp64 group sums)
+ *  2  k_gn_small: statistics + apply in one block per image; needs HW <= 64
+ *  3  k_gn_apply from the producers' quad statistics qs0 / qs1 [B][C0/4][2] / [B][C1/4][2] fp64 {sum, sum of squares}
+ *     (ddpm_gn_epi); needs C % 128 == 0
+ *  4  k_gn_prep: K only, from the quad statistics (y is not written); needs C % 128 == 0
+ * Outputs: y bf16 [B][HW][C] = act(gn(x)) * keep / (1 - drop_p);  K f32 [B][4][C] = {rstd*gamma, beta - mean*rstd*gamma, rstd,
+ * mean*rstd} per (image, channel).  Dropout is on when drop_p > 0 and seed != 0: the keep bit of element (b, p, c) is a Philox
+ * draw keyed by (seed, layer) at counter (b*HW + p)*C + c; mask (optional) [B][HW][C/8] receives the keep bits, bit e of byte
+ * (b, p, o) = channel 8*o + e. */
+typedef struct ddpm_gn_desc {
+    int route, B, HW, C0, C1;
+    const void* x0; const void* x1;
+    const float* gamma; const float* beta;
+    int silu; float drop_p; uint64_t seed; uint32_t layer;
+    unsigned char* mask;
+    const double* qs0; const double* qs1;
+    void* y; float* K;
+    void* scratch;
+} ddpm_gn_desc;
+/* Backward of the forward above (autograd of unet.py:83-84 with the saved K and mask): with dn = dy * keep/(1 - drop_p) * act'(y),
+ *   dx = rstd*gamma*dn - P*x - Q (+ addend) written to dx0 / dx1 (acc0 / acc1 != 0: added to what is there),
+ *   dgamma += sum dn*xhat,  dbeta += sum dn  (over images and pixels).
+ * dn_inplace != 0 overwrites dy with bf16(dn) in the first pass.  drop_p > 0 needs the forward's mask.
+ * Column sums of dx (any of them may be NULL): cs_per_img[b][cs_ld] +=, cs_total[c] +=, cs_total2[c] +=. */
+typedef struct ddpm_gn_bwd_desc {
+    int B, HW, C0, C1;
+    const void* x0; const void* x1;
+    void* dy;
+    const float* K; const float* gamma;
+    float* dgamma; float* dbeta;
+    void* dx0; void* dx1; int acc0, acc1;
+    const void* addend;
+    int silu; float drop_p; const unsigned char* mask;
+    int dn_inplace;
+    float* cs_per_img; int cs_ld; float* cs_total; float* cs_total2;
+    void* scratch;
+} ddpm_gn_bwd_desc;
+long long ddpm_gn_scratch_bytes(int B, int C);
+int ddpm_groupnorm_fwd_run(const ddpm_gn_desc* d, void* stream);
+int ddpm_groupnorm_bwd_run(const ddpm_gn_bwd_desc* d, void* stream);
+/* Bias gradients (autograd of the conv / linear bias): column sums of dy bf16 [B][HW][C] over its first C_valid channels,
+ * per_img[b][ld] += (optional), total[c] += (optional), total2[c] += (optional).  C a multiple of 8, any width. */
+int ddpm_colsum_run(const void* dy, float* per_img, int ld, float* total, float* total2, int B, int HW, int C, int C_valid, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * UNet engine.  replaces: UNet.__init__/forward (ddpm_torch/models/unet.py:96-233), its autograd backward,
  * and the model-side half of GaussianDiffusion.train_losses / p_sample_step (diffusion.py:107-158,217-243).
  */

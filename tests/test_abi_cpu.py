@@ -33,16 +33,21 @@ def test_library_exports_every_declared_symbol(L):
 
 def test_struct_layouts_match_header():
     from ddpm_torch_b200 import _lib
-    src = '#include "include/ddpm_b200.h"\n#include <stdio.h>\n#include <stddef.h>\nint main(){printf("%zu %zu %zu %zu %zu %zu %zu", sizeof(ddpm_gemm_desc), sizeof(ddpm_unet_cfg), sizeof(ddpm_opt_cfg), sizeof(ddpm_halo_desc), sizeof(ddpm_gn_epi), offsetof(ddpm_gemm_desc, gn), offsetof(ddpm_halo_desc, gn));}'
+    src = ('#include "include/ddpm_b200.h"\n#include <stdio.h>\n#include <stddef.h>\nint main(){printf("%zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu", '
+           'sizeof(ddpm_gemm_desc), sizeof(ddpm_unet_cfg), sizeof(ddpm_opt_cfg), sizeof(ddpm_halo_desc), sizeof(ddpm_gn_epi), '
+           'offsetof(ddpm_gemm_desc, gn), offsetof(ddpm_halo_desc, gn), sizeof(ddpm_gn_desc), sizeof(ddpm_gn_bwd_desc), '
+           'offsetof(ddpm_gn_desc, seed), offsetof(ddpm_gn_bwd_desc, scratch));}')
     import subprocess, tempfile
     with tempfile.TemporaryDirectory() as td:
         c = os.path.join(td, "s.c"); open(c, "w").write(src)
         exe = os.path.join(td, "s")
         subprocess.check_call(["gcc", "-I", ROOT, c, "-o", exe], cwd=ROOT)
-        a, b, c_, hd, ge, og, oh = map(int, subprocess.check_output([exe]).split())
+        a, b, c_, hd, ge, og, oh, gd, gbd, o_seed, o_scr = map(int, subprocess.check_output([exe]).split())
     assert a == C.sizeof(_lib.GemmDesc) and b == C.sizeof(_lib.UnetCfg) and c_ == C.sizeof(_lib.OptCfg)
     assert hd == C.sizeof(_lib.HaloDesc) and ge == C.sizeof(_lib.GnEpi)
     assert og == _lib.GemmDesc.gn.offset and oh == _lib.HaloDesc.gn.offset
+    assert gd == C.sizeof(_lib.GnDesc) and gbd == C.sizeof(_lib.GnBwdDesc)
+    assert o_seed == _lib.GnDesc.seed.offset and o_scr == _lib.GnBwdDesc.scratch.offset
 
 
 def test_no_gpu_means_error_not_fallback(L):

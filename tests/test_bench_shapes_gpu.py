@@ -335,6 +335,22 @@ def test_celeba64_config_fwd_bwd():
     grads_vs_oracle(m, sd, CELEBA64_CFG, x0, t, noise, "celeba 64x64 bs=8 train", chunk=4)
 
 
+WIDE_ATTN_CFG = dict(in_channels=3, hid_channels=256, out_channels=3, ch_multipliers=(1, 2, 4), num_res_blocks=2,
+                     apply_attn=(False, False, True), drop_rate=0.0)
+
+
+def test_wide_attention_config_fwd_bwd():
+    """hid 256, ch_mult (1, 2, 4), attention at the 1024-channel level: project_in's bias gradient is a column sum over
+    3 * 1024 channels (k_colsum in 2048-channel slices) and the up path's widest GroupNorm concat is 1024 + 1024.
+    Loss and all gradients at bs=2, 32x32."""
+    m, sd = build(WIDE_ATTN_CFG, 31, train=True)
+    g = torch.Generator(DEV).manual_seed(31)
+    x0 = torch.rand(2, 3, 32, 32, device=DEV, generator=g) * 2 - 1
+    t = torch.randint(1000, (2,), device=DEV, generator=g)
+    noise = torch.randn(2, 3, 32, 32, device=DEV, generator=g)
+    grads_vs_oracle(m, sd, WIDE_ATTN_CFG, x0, t, noise, "hid 256 (1, 2, 4) attention at 1024 channels, bs=2 train")
+
+
 def test_gradient_chunks_tile_the_flat_buffer(golden):
     """data-parallel seam: the backward completes the flat gradient buffer in contiguous chunks (ddpm_unet_grad_chunks) that
     tile it exactly; waiting for a chunk's event on another stream and reading the chunk there sees the final gradients."""
