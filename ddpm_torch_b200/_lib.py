@@ -112,6 +112,7 @@ def lib():
             "ddpm_groupnorm_bwd_run": ([C.POINTER(GnBwdDesc), vp], i32),
             "ddpm_colsum_run": ([vp, vp, i32, vp, vp, i32, i32, i32, i32, vp], i32),
             "ddpm_unet_create": ([C.POINTER(UnetCfg), C.POINTER(vp)], i32),
+            "ddpm_unet_create_ex": ([C.POINTER(UnetCfg), i32, C.POINTER(vp)], i32),
             "ddpm_unet_destroy": ([vp], None),
             "ddpm_unet_num_params": ([vp], i32),
             "ddpm_unet_param_info": ([vp, i32, C.POINTER(C.c_char_p), C.POINTER(i32), C.POINTER(i32 * 4), C.POINTER(i64)], i32),
@@ -149,7 +150,7 @@ def lib():
 
 EXPORTS = ["ddpm_last_error", "ddpm_runtime_check", "ddpm_device_error_flag", "ddpm_gemm_run", "ddpm_conv_halo_run", "ddpm_attn_fused_run", "ddpm_attn_fused_bwd_run",
            "ddpm_gn_scratch_bytes", "ddpm_groupnorm_fwd_run", "ddpm_groupnorm_bwd_run", "ddpm_colsum_run",
-           "ddpm_unet_create", "ddpm_unet_destroy", "ddpm_unet_num_params", "ddpm_unet_param_info",
+           "ddpm_unet_create", "ddpm_unet_create_ex", "ddpm_unet_destroy", "ddpm_unet_num_params", "ddpm_unet_param_info",
            "ddpm_unet_flat_elems", "ddpm_unet_workspace_bytes", "ddpm_unet_plan", "ddpm_unet_repack",
            "ddpm_unet_forward", "ddpm_unet_backward", "ddpm_train_forward", "ddpm_train_backward",
            "ddpm_sampler_setup", "ddpm_sampler_reset", "ddpm_sampler_step", "ddpm_sampler_step_pred",

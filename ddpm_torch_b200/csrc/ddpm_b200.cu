@@ -171,14 +171,17 @@ int ddpm_colsum_run(const void* dy, float* per_img, int ld, float* total, float*
 }
 
 // ------------------------------------------------------------------------------------------------ UNet engine
-int ddpm_unet_create(const ddpm_unet_cfg* cfg, ddpm_unet** out) {
+int ddpm_unet_create(const ddpm_unet_cfg* cfg, ddpm_unet** out) { return ddpm_unet_create_ex(cfg, 1, out); }
+int ddpm_unet_create_ex(const ddpm_unet_cfg* cfg, int resample_with_conv, ddpm_unet** out) {
     if (!cfg || !out) return fail(-30, "null argument");
+    if (resample_with_conv != 0 && resample_with_conv != 1) return fail(-30, "resample_with_conv must be 0 or 1 (got %d)", resample_with_conv);
     if (cfg->levels < 1 || cfg->levels > 8) return fail(-30, "levels must be 1..8");
     if (cfg->hid_channels <= 0 || cfg->hid_channels % 32) return fail(-30, "hid_channels must be a positive multiple of 32");
     if (cfg->num_res_blocks < 1) return fail(-30, "num_res_blocks must be >= 1");
     ddpm_unet* h = new (std::nothrow) ddpm_unet();
     if (!h) return fail(-30, "out of host memory");
     h->e.cfg = *cfg;
+    h->e.resample_with_conv = resample_with_conv != 0;
     if (h->e.cfg.temb_dim <= 0) h->e.cfg.temb_dim = 4 * cfg->hid_channels;
     h->e.register_params();
     *out = h;

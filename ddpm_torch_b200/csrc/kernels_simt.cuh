@@ -1286,32 +1286,113 @@ __global__ void __launch_bounds__(256) k_attn16_bwd(const bf16* __restrict__ qkv
     }
 }
 
-// ============================================================================ nearest 2x upsample (unet.py:199) and its adjoint
-__global__ void k_upsample2x(const bf16* __restrict__ in, bf16* __restrict__ out, int B, int H, int W, int C) {
+// ============================================================================ nearest 2x upsample (unet.py:199), 2x2 average pool
+// (unet.py:168, AvgPool2d(2)) and their adjoints: one kernel per direction, in [B][H][W][C] -> out [B][2H][2W][C] and back.
+// k_upsample2x:      out (+)= scale * nearest(in)          upsample forward (scale 1), pool backward (scale 1/4)
+//   qs_out:          quad statistics of out (null = off): 4 x those of in when qs_in is set (every low-res pixel appears four
+//                    times), else reduced from out itself into the zeroed qs_out (C % 32 == 0)
+// k_upsample2x_bwd:  in (+)= scale * (sum of each 2x2 window of out)   upsample backward (scale 1), pool forward (scale 1/4)
+//   qstats:          quad statistics of the written low-res tensor (gn_epilogue.cuh; zeroed, C % 32 == 0, H*W % 32 == 0)
+__global__ void k_upsample2x(const bf16* __restrict__ in, bf16* __restrict__ out, int B, int H, int W, int C, float scale, int accumulate,
+                             const double* __restrict__ qs_in, double* __restrict__ qs_out) {
     pdl_entry();
     const int oct = C >> 3;
+    const long long stride = (long long)gridDim.x * blockDim.x, tid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (qs_out && qs_in) for (long long i = tid; i < (long long)B * (C >> 2) * 2; i += stride) qs_out[i] = 4.0 * qs_in[i];
+    if (qs_out && !qs_in) {
+        // no input statistics: reduce the output itself (zeroed qs_out, C % 32 == 0, 4*H*W % 32 == 0), one warp = 32 consecutive
+        // output pixels of one image x one 32-channel slab, lane = pixel (the epilogues' butterfly, epi_quad_stats)
+        const int lane = threadIdx.x & 31, slabs = C >> 5;
+        const long long nwarps = (long long)B * 4 * H * W / 32 * slabs;
+        for (long long wi = tid >> 5; wi < nwarps; wi += stride >> 5) {
+            const long long pix = (wi / slabs) * 32 + lane; const int sl = (int)(wi % slabs);
+            const int b = (int)(pix / (4 * H * W)), r = (int)(pix % (4 * H * W)), y = r / (2 * W), x = r % (2 * W);
+            const uint4* s = reinterpret_cast<const uint4*>(in) + (((long long)b * H + (y >> 1)) * W + (x >> 1)) * oct + sl * 4;
+            uint4* d = reinterpret_cast<uint4*>(out) + pix * oct + sl * 4;
+            float f[32];
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                float v[8], g[8];
+                unpack8(__ldg(s + k), v);
+                if (accumulate) unpack8(d[k], g);
+#pragma unroll
+                for (int e = 0; e < 8; ++e) { v[e] *= scale; if (accumulate) v[e] += g[e]; f[8 * k + e] = v[e]; }
+                d[k] = pack8(v);
+            }
+            epi_quad_stats(f, true, qs_out + ((long long)b * (C >> 2) + sl * 8) * 2, lane);
+        }
+        return;
+    }
     const long long total = (long long)B * 4 * H * W * oct;
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const bool copy = scale == 1.f && !accumulate;
+    for (long long i = tid; i < total; i += stride) {
         const long long pix = i / oct; const int o = (int)(i % oct);
         const int b = (int)(pix / (4 * H * W)), r = (int)(pix % (4 * H * W)), y = r / (2 * W), x = r % (2 * W);
-        reinterpret_cast<uint4*>(out)[i] = __ldg(reinterpret_cast<const uint4*>(in) + (((long long)b * H + (y >> 1)) * W + (x >> 1)) * oct + o);
+        const uint4 v = __ldg(reinterpret_cast<const uint4*>(in) + (((long long)b * H + (y >> 1)) * W + (x >> 1)) * oct + o);
+        if (copy) { reinterpret_cast<uint4*>(out)[i] = v; continue; }
+        float f[8];
+        unpack8(v, f);
+#pragma unroll
+        for (int e = 0; e < 8; ++e) f[e] *= scale;
+        if (accumulate) {
+            float g[8];
+            unpack8(reinterpret_cast<const uint4*>(out)[i], g);
+#pragma unroll
+            for (int e = 0; e < 8; ++e) f[e] += g[e];
+        }
+        reinterpret_cast<uint4*>(out)[i] = pack8(f);
     }
 }
-__global__ void k_upsample2x_bwd(const bf16* __restrict__ dout, bf16* __restrict__ din, int B, int H, int W, int C, int accumulate) {
+__global__ void k_upsample2x_bwd(const bf16* __restrict__ dout, bf16* __restrict__ din, int B, int H, int W, int C, int accumulate, float scale,
+                                 double* __restrict__ qstats) {
     pdl_entry();
     const int oct = C >> 3;
+    const long long stride = (long long)gridDim.x * blockDim.x, tid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const uint4* src = reinterpret_cast<const uint4*>(dout);
+    if (qstats) {
+        // one warp = 32 consecutive low-res pixels (one image: H*W % 32 == 0) x one 32-channel slab; lane = pixel, so that the
+        // epilogues' butterfly (epi_quad_stats) reduces the warp's pixels per quad
+        const int lane = threadIdx.x & 31, slabs = C >> 5;
+        const long long nwarps = (long long)B * H * W / 32 * slabs;
+        for (long long wi = tid >> 5; wi < nwarps; wi += stride >> 5) {
+            const long long pix = (wi / slabs) * 32 + lane; const int sl = (int)(wi % slabs);
+            const int b = (int)(pix / (H * W)), r = (int)(pix % (H * W)), y = r / W, x = r % W;
+            float f[32];
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                float s[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {
+                    float g[8];
+                    unpack8(__ldg(src + (((long long)b * 2 * H + 2 * y + (q >> 1)) * 2 * W + 2 * x + (q & 1)) * oct + sl * 4 + k), g);
+#pragma unroll
+                    for (int e = 0; e < 8; ++e) s[e] += g[e];
+                }
+                uint4* d = reinterpret_cast<uint4*>(din) + pix * oct + sl * 4 + k;
+                float g[8];
+                if (accumulate) unpack8(*d, g);
+#pragma unroll
+                for (int e = 0; e < 8; ++e) { s[e] *= scale; if (accumulate) s[e] += g[e]; f[8 * k + e] = s[e]; }
+                *d = pack8(s);
+            }
+            epi_quad_stats(f, true, qstats + ((long long)b * (C >> 2) + sl * 8) * 2, lane);
+        }
+        return;
+    }
     const long long total = (long long)B * H * W * oct;
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    for (long long i = tid; i < total; i += stride) {
         const long long pix = i / oct; const int o = (int)(i % oct);
         const int b = (int)(pix / (H * W)), r = (int)(pix % (H * W)), y = r / W, x = r % W;
         float s[8] = {0, 0, 0, 0, 0, 0, 0, 0};
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
             float f[8];
-            unpack8(__ldg(reinterpret_cast<const uint4*>(dout) + (((long long)b * 2 * H + 2 * y + (q >> 1)) * 2 * W + 2 * x + (q & 1)) * oct + o), f);
+            unpack8(__ldg(src + (((long long)b * 2 * H + 2 * y + (q >> 1)) * 2 * W + 2 * x + (q & 1)) * oct + o), f);
 #pragma unroll
             for (int e = 0; e < 8; ++e) s[e] += f[e];
         }
+#pragma unroll
+        for (int e = 0; e < 8; ++e) s[e] *= scale;
         if (accumulate) {
             float f[8];
             unpack8(reinterpret_cast<const uint4*>(din)[i], f);

@@ -97,6 +97,7 @@ static inline int launch_colsum(const bf16* dy, float* per_img, int ld, float* t
 
 struct UnetEngine {
     ddpm_unet_cfg cfg;
+    bool resample_with_conv = true;       // false: AvgPool2d(2) / bare nearest x2 instead of the resample convs (unet.py:164-170,199-202)
     std::vector<ParamInfo> params;
     std::map<std::string, int> pidx;
     long long flat_elems = 0;
@@ -158,7 +159,7 @@ struct UnetEngine {
             const std::string p = "downsamples.level_" + std::to_string(i);
             reg_block(p + ".0", prev, cur, cfg.attn[i]);
             for (int j = 1; j < nrb; ++j) reg_block(p + "." + std::to_string(j), cur, cur, cfg.attn[i]);
-            if (i != L - 1) reg_conv(p + "." + std::to_string(nrb) + ".1", cur, cur, 3);
+            if (i != L - 1 && resample_with_conv) reg_conv(p + "." + std::to_string(nrb) + ".1", cur, cur, 3);
         }
         const int mid = chs(L - 1);
         reg_res("middle.0", mid, mid); reg_attn("middle.1", mid); reg_res("middle.2", mid, mid);
@@ -168,7 +169,7 @@ struct UnetEngine {
             reg_block(p + ".0", prev + cur, cur, cfg.attn[i]);
             for (int j = 1; j < nrb; ++j) reg_block(p + "." + std::to_string(j), 2 * cur, cur, cfg.attn[i]);
             reg_block(p + "." + std::to_string(nrb), nxt + cur, cur, cfg.attn[i]);
-            if (i != 0) reg_conv(p + "." + std::to_string(nrb + 1) + ".1", cur, cur, 3);
+            if (i != 0 && resample_with_conv) reg_conv(p + "." + std::to_string(nrb + 1) + ".1", cur, cur, 3);
         }
         reg_gn("out_conv.0", ch); reg_conv("out_conv.2", ch, cfg.out_channels, 3);
         layout_params();
@@ -568,6 +569,8 @@ struct UnetEngine {
     T4 attn_block(const std::string& p, const T4& x);
     T4 down_conv(const std::string& p, const T4& x);
     T4 up_conv(const std::string& p, const T4& x);
+    T4 down_pool(const std::string& p, const T4& x);
+    T4 up_nearest(const std::string& p, const T4& x);
     void bmm(std::vector<Op>& L, const std::string& name, int form, const bf16* A, long long lda, long long sa, const bf16* Bp, long long ldb, long long sb,
              void* C, long long ldc, long long sc, bool c_f32, int nb, int T, int Cc, float alpha, double* fl_acc);
     int plan(int B_, int H_, int W_, bool train_, bool dry_);

@@ -316,7 +316,7 @@ inline T4 UnetEngine::up_conv(const std::string& p, const T4& x) {
     }
     T4 up = newT(Bn, 2 * h, 2 * w, C);
     { const bf16* src = bp(x); bf16* dst = bp(up); const int n = grid_for((long long)Bn * 4 * h * w * (C / 8));
-      push(fwd_ops, p + ".upsample", 0, [=](cudaStream_t st) { launch_k(k_upsample2x, n, 256, 0, st, src, dst, Bn, h, w, C); return (int)cudaGetLastError(); }); }
+      push(fwd_ops, p + ".upsample", 0, [=](cudaStream_t st) { launch_k(k_upsample2x, n, 256, 0, st, src, dst, Bn, h, w, C, 1.f, 0, (const double*)nullptr, (double*)nullptr); return (int)cudaGetLastError(); }); }
     const Packed pk = pack_conv(p, C, C, 3, 0, true, true);
     T4 out = newT(Bn, 2 * h, 2 * w, C);
     { ConvSpec c; c.name = p; c.in = one(up); c.wp = pk.fwd; c.ldw = pk.ld_f; c.bias = PP(p + ".bias"); c.out = out; c.Co = C; c.Ho = 2 * h; c.Wo = 2 * w;
@@ -331,7 +331,52 @@ inline T4 UnetEngine::up_conv(const std::string& p, const T4& x) {
         wgrad_op(p + ".wgrad", dY, one(up), 3, 1, MAP_NORMAL, GP(p + ".weight"), C);
         bool first = true; const T4 dx = grad_of(x, &first);
         const bf16* src = bp(dUp); bf16* dst = bp(dx); const int n = grid_for((long long)Bn * h * w * (C / 8)); const int acc = first ? 0 : 1;
-        push(bwd_ops, p + ".upsample_bwd", 0, [=](cudaStream_t st) { launch_k(k_upsample2x_bwd, n, 256, 0, st, src, dst, Bn, h, w, C, acc); return (int)cudaGetLastError(); });
+        push(bwd_ops, p + ".upsample_bwd", 0, [=](cudaStream_t st) { launch_k(k_upsample2x_bwd, n, 256, 0, st, src, dst, Bn, h, w, C, acc, 1.f, (double*)nullptr); return (int)cudaGetLastError(); });
+    });
+    return out;
+}
+
+// resample_with_conv=False (unet.py:168-169): AvgPool2d(2), y = bf16(sum of the 2x2 window / 4) in fp32.  Like the stride-2 conv it
+// replaces, it hands the next norm1 (and, as a skip, the up path's concat) the quad statistics of its output when the shape allows.
+inline T4 UnetEngine::down_pool(const std::string& p, const T4& x) {
+    const int C = x.C, Bn = x.B, h = x.H / 2, w = x.W / 2;
+    T4 out = newT(Bn, h, w, C);
+    double* qs = nullptr;
+    static const bool no_fuse = getenv("DDPM_NO_GN_EPI") != nullptr;
+    if (!no_fuse && C % 32 == 0 && (h * w) % 32 == 0) { out.qs = (long long)zero_fwd((size_t)Bn * (C / 4) * 2 * 8); qs = at<double>((size_t)out.qs); }
+    { const bf16* src = bp(x); bf16* dst = bp(out);
+      const int n = qs ? grid_for((long long)Bn * h * w * (C / 32)) : grid_for((long long)Bn * h * w * (C / 8));
+      push(fwd_ops, p + ".pool", 0, [=](cudaStream_t st) { launch_k(k_upsample2x_bwd, n, 256, 0, st, src, dst, Bn, h, w, C, 0, 0.25f, qs); return (int)cudaGetLastError(); }); }
+    if (!train) return out;
+    tape_push([=]() {
+        const T4 dY = grad_of(out, nullptr);
+        bool first = true; const T4 dx = grad_of(x, &first);
+        const bf16* src = bp(dY); bf16* dst = bp(dx); const int n = grid_for((long long)Bn * 4 * h * w * (C / 8)); const int acc = first ? 0 : 1;
+        push(bwd_ops, p + ".pool_bwd", 0, [=](cudaStream_t st) {
+            launch_k(k_upsample2x, n, 256, 0, st, src, dst, Bn, h, w, C, 0.25f, acc, (const double*)nullptr, (double*)nullptr); return (int)cudaGetLastError(); });
+    });
+    return out;
+}
+
+// resample_with_conv=False (unet.py:199-202): nearest x2 alone, materialised in training and inference plans.  Its quad statistics
+// are 4x those of the low-res input (every pixel appears four times) when the producer delivered them, else the kernel reduces its
+// own output (4x4 maps, split-K producers), so the following concat keeps the one-pass GroupNorm wherever the 3x3 conv gave it.
+inline T4 UnetEngine::up_nearest(const std::string& p, const T4& x) {
+    const int C = x.C, Bn = x.B, h = x.H, w = x.W;
+    T4 out = newT(Bn, 2 * h, 2 * w, C);
+    const double* qs_in = nullptr; double* qs_out = nullptr;
+    static const bool no_fuse = getenv("DDPM_NO_GN_EPI") != nullptr;
+    if (x.qs >= 0) { out.qs = (long long)alloc((size_t)Bn * (C / 4) * 2 * 8); qs_in = at<double>((size_t)x.qs); qs_out = at<double>((size_t)out.qs); }
+    else if (!no_fuse && C % 32 == 0 && (4 * h * w) % 32 == 0) { out.qs = (long long)zero_fwd((size_t)Bn * (C / 4) * 2 * 8); qs_out = at<double>((size_t)out.qs); }
+    { const bf16* src = bp(x); bf16* dst = bp(out);
+      const int n = (qs_out && !qs_in) ? grid_for((long long)Bn * 4 * h * w * (C / 32)) : grid_for((long long)Bn * 4 * h * w * (C / 8));
+      push(fwd_ops, p + ".upsample", 0, [=](cudaStream_t st) { launch_k(k_upsample2x, n, 256, 0, st, src, dst, Bn, h, w, C, 1.f, 0, qs_in, qs_out); return (int)cudaGetLastError(); }); }
+    if (!train) return out;
+    tape_push([=]() {
+        const T4 dY = grad_of(out, nullptr);
+        bool first = true; const T4 dx = grad_of(x, &first);
+        const bf16* src = bp(dY); bf16* dst = bp(dx); const int n = grid_for((long long)Bn * h * w * (C / 8)); const int acc = first ? 0 : 1;
+        push(bwd_ops, p + ".upsample_bwd", 0, [=](cudaStream_t st) { launch_k(k_upsample2x_bwd, n, 256, 0, st, src, dst, Bn, h, w, C, acc, 1.f, (double*)nullptr); return (int)cudaGetLastError(); });
     });
     return out;
 }
@@ -623,7 +668,10 @@ inline int UnetEngine::plan(int B_, int H_, int W_, bool train_, bool dry_) {
         const std::string p = "downsamples.level_" + std::to_string(i);
         cur_tag = "d" + std::to_string(i);
         for (int j = 0; j < nrb; ++j) hs.push_back(block(p + "." + std::to_string(j), one(hs.back()), chs(i), cfg.attn[i] != 0));
-        if (i != L - 1) hs.push_back(down_conv(p + "." + std::to_string(nrb) + ".1", hs.back()));
+        if (i != L - 1) {
+            const std::string q = p + "." + std::to_string(nrb);
+            hs.push_back(resample_with_conv ? down_conv(q + ".1", hs.back()) : down_pool(q, hs.back()));
+        }
     }
     // ---- middle (unet.py:132-136,221)
     T4 h = hs.back();
@@ -639,7 +687,10 @@ inline int UnetEngine::plan(int B_, int H_, int W_, bool train_, bool dry_) {
             Src s; s.t0 = h; s.t1 = hs.back(); s.two = true; hs.pop_back();
             h = block(p + "." + std::to_string(j), s, chs(i), cfg.attn[i] != 0);
         }
-        if (i != 0) h = up_conv(p + "." + std::to_string(nrb + 1) + ".1", h);
+        if (i != 0) {
+            const std::string q = p + "." + std::to_string(nrb + 1);
+            h = resample_with_conv ? up_conv(q + ".1", h) : up_nearest(q, h);
+        }
     }
     if (blk != nblocks) return fail(-31, "internal: block count mismatch %d vs %d", blk, nblocks);
     // ---- out_conv (unet.py:138-142,232): GN -> SiLU -> conv3x3 (C -> Cout<=4) -> NCHW fp32

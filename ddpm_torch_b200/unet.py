@@ -31,8 +31,6 @@ class UNet(nn.Module):
     def __init__(self, in_channels, hid_channels, out_channels, ch_multipliers, num_res_blocks, apply_attn,
                  time_embedding_dim=None, drop_rate=0., resample_with_conv=True):
         super().__init__()
-        if not resample_with_conv:
-            raise NotImplementedError("resample_with_conv=False (AvgPool/plain Upsample) is outside the accelerated path")
         levels = len(ch_multipliers)
         if isinstance(apply_attn, bool):
             apply_attn = [apply_attn] * levels
@@ -40,7 +38,7 @@ class UNet(nn.Module):
         self.ch_multipliers, self.apply_attn = tuple(ch_multipliers), tuple(bool(a) for a in apply_attn)
         self.num_res_blocks, self.levels = num_res_blocks, levels
         self.time_embedding_dim = time_embedding_dim or 4 * hid_channels
-        self.drop_rate, self.resample_with_conv = drop_rate, resample_with_conv
+        self.drop_rate, self.resample_with_conv = drop_rate, bool(resample_with_conv)
 
         cfg = _lib.UnetCfg()
         cfg.in_channels, cfg.hid_channels, cfg.out_channels = in_channels, hid_channels, out_channels
@@ -52,7 +50,7 @@ class UNet(nn.Module):
         L = _lib.lib()
         self._cfg = cfg
         self._h = C.c_void_p()
-        _lib.check(L.ddpm_unet_create(C.byref(cfg), C.byref(self._h)), "unet_create")
+        _lib.check(L.ddpm_unet_create_ex(C.byref(cfg), int(self.resample_with_conv), C.byref(self._h)), "unet_create")
         self._aux = {}                      # auxiliary inference plans (extra handles over the SAME flat parameters)
 
         # parameter inventory from the engine (reference registration order)
@@ -220,7 +218,7 @@ class UNet(nn.Module):
         if a is None or a["key"] != key:
             if a is None:
                 h = C.c_void_p()
-                _lib.check(L.ddpm_unet_create(C.byref(self._cfg), C.byref(h)), "unet_create")
+                _lib.check(L.ddpm_unet_create_ex(C.byref(self._cfg), int(self.resample_with_conv), C.byref(h)), "unet_create")
                 a = {"h": h, "ws": None, "key": None, "ver": None}
                 self._aux[idx] = a
             need = L.ddpm_unet_workspace_bytes(a["h"], B, H, W, 0)

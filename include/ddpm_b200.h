@@ -168,7 +168,11 @@ typedef struct ddpm_unet_cfg {          /* mirrors UNet(in_channels, hid_channel
 } ddpm_unet_cfg;
 typedef struct ddpm_unet ddpm_unet;
 
+/* ddpm_unet_create(cfg, out) is ddpm_unet_create_ex(cfg, 1, out).  resample_with_conv (unet.py:106,164-170,199-202):
+ * 1 = SamePad2d(3, 2) + stride-2 3x3 conv down, nearest x2 + 3x3 conv up;  0 = AvgPool2d(2) down, bare nearest x2 up, and the
+ * resample convs are absent from the parameter inventory.  Any other value is refused before anything is allocated. */
 int  ddpm_unet_create(const ddpm_unet_cfg* cfg, ddpm_unet** out);
+int  ddpm_unet_create_ex(const ddpm_unet_cfg* cfg, int resample_with_conv, ddpm_unet** out);
 void ddpm_unet_destroy(ddpm_unet* h);
 /* Parameter inventory in the reference's state_dict order (unet.py registration order). Offsets (in fp32 elements)
  * address the FLAT parameter / gradient buffers the caller owns; each tensor is OIHW / [out,in] fp32 as in the reference. */
