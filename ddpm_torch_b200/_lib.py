@@ -122,6 +122,8 @@ def lib():
             "ddpm_unet_repack": ([vp, vp], i32),
             "ddpm_unet_forward": ([vp, vp, vp, vp, u64, vp], i32),
             "ddpm_unet_backward": ([vp, vp, vp], i32),
+            "ddpm_unet_backward_ex": ([vp, vp, vp, i32, vp], i32),
+            "ddpm_unet_backward_launches": ([vp, i32, i32], i32),
             "ddpm_train_forward": ([vp, vp, vp, vp, vp, vp, vp, u64, vp], i32),
             "ddpm_train_backward": ([vp, vp, vp], i32),
             "ddpm_sampler_setup": ([vp, i32, vp, vp], i32),
@@ -152,7 +154,7 @@ EXPORTS = ["ddpm_last_error", "ddpm_runtime_check", "ddpm_device_error_flag", "d
            "ddpm_gn_scratch_bytes", "ddpm_groupnorm_fwd_run", "ddpm_groupnorm_bwd_run", "ddpm_colsum_run",
            "ddpm_unet_create", "ddpm_unet_create_ex", "ddpm_unet_destroy", "ddpm_unet_num_params", "ddpm_unet_param_info",
            "ddpm_unet_flat_elems", "ddpm_unet_workspace_bytes", "ddpm_unet_plan", "ddpm_unet_repack",
-           "ddpm_unet_forward", "ddpm_unet_backward", "ddpm_train_forward", "ddpm_train_backward",
+           "ddpm_unet_forward", "ddpm_unet_backward", "ddpm_unet_backward_ex", "ddpm_unet_backward_launches", "ddpm_train_forward", "ddpm_train_backward",
            "ddpm_sampler_setup", "ddpm_sampler_reset", "ddpm_sampler_step", "ddpm_sampler_step_pred",
            "ddpm_bpd_setup", "ddpm_bpd_reset", "ddpm_bpd_step", "ddpm_unet_grad_chunks", "ddpm_unet_wait_grad_chunk", "ddpm_unet_plan_stats",
            "ddpm_unet_launches_per_forward", "ddpm_unet_launch_counts", "ddpm_opt_step", "ddpm_to_uint8_nhwc"]

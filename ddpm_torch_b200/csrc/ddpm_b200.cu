@@ -243,13 +243,25 @@ int ddpm_unet_forward(ddpm_unet* h, const float* x, const int64_t* t, float* eps
     e.x_in = x; e.t_in = reinterpret_cast<const long long*>(t); e.eps_dst = eps; e.drop_seed = dropout_seed;
     return e.run_list(e.fwd_ops, static_cast<cudaStream_t>(stream));
 }
-int ddpm_unet_backward(ddpm_unet* h, const float* d_eps, void* stream) {
+int ddpm_unet_backward(ddpm_unet* h, const float* d_eps, void* stream) { return ddpm_unet_backward_ex(h, d_eps, nullptr, 1, stream); }
+int ddpm_unet_backward_ex(ddpm_unet* h, const float* d_eps, float* dx, int param_grads, void* stream) {
+    if (param_grads != 0 && param_grads != 1) return fail(-30, "ddpm_unet_backward_ex: param_grads must be 0 or 1 (got %d)", param_grads);
+    if (!param_grads && !dx) return fail(-30, "ddpm_unet_backward_ex: nothing to compute (param_grads = 0 and dx = NULL)");
     NEED_PLAN(h);
     UnetEngine& e = h->e;
     if (!e.train) return fail(-33, "plan was built without training");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    e.deps_src = d_eps;
-    return e.run_list(e.bwd_ops, st);
+    e.deps_src = d_eps; e.dx_dst = dx; e.bwd_dx = dx != nullptr; e.bwd_params = param_grads != 0;
+    const int rc = e.run_list(e.bwd_ops, st);
+    e.chunks_current = e.bwd_params;
+    e.dx_dst = nullptr; e.bwd_dx = false; e.bwd_params = true;
+    return rc;
+}
+int ddpm_unet_backward_launches(const ddpm_unet* h, int want_dx, int param_grads) {
+    if (!h || !h->e.train) return fail(-33, "ddpm_unet_backward_launches: no training plan");
+    if ((want_dx != 0 && want_dx != 1) || (param_grads != 0 && param_grads != 1)) return fail(-30, "ddpm_unet_backward_launches: flags must be 0 or 1");
+    if (!want_dx && !param_grads) return fail(-30, "ddpm_unet_backward_launches: nothing to compute (want_dx = 0 and param_grads = 0)");
+    return h->e.count_bwd_launches(want_dx != 0, param_grads != 0);
 }
 int ddpm_train_forward(ddpm_unet* h, const float* x0, const int64_t* t, const float* noise, const float* tab_a, const float* tab_s,
                        float* losses, uint64_t dropout_seed, void* stream) {
@@ -284,6 +296,7 @@ int ddpm_train_backward(ddpm_unet* h, const float* gscale, void* stream) {
     launch_k(k_mse_grad, grid_for(total), 256, 0, st, e.at<float>(e.eps_off), h->train_target, gscale, e.at<float>(e.deps_off), per_img, total);
     DDPM_CUDA_OK(cudaGetLastError());
     e.deps_src = e.at<float>(e.deps_off);
+    e.chunks_current = true;
     return e.run_list(e.bwd_ops, st);
 }
 
@@ -463,6 +476,7 @@ int ddpm_unet_grad_chunks(const ddpm_unet* h, int max_n, long long* lo, long lon
 int ddpm_unet_wait_grad_chunk(ddpm_unet* h, int i, void* stream) {
     NEED_PLAN(h);
     if (i < 0 || i >= (int)h->e.chunks.size() || !h->e.chunks[i].ev) return fail(-30, "gradient chunk index out of range");
+    if (!h->e.chunks_current) return fail(-33, "the most recent backward computed no parameter gradients: it recorded no gradient chunk");
     DDPM_CUDA_OK(cudaStreamWaitEvent(static_cast<cudaStream_t>(stream), h->e.chunks[i].ev, 0));
     return 0;
 }
@@ -478,7 +492,7 @@ int ddpm_unet_plan_stats(const ddpm_unet* h, int* n_fwd, int* n_bwd, int* n_tc, 
 int ddpm_unet_launches_per_forward(const ddpm_unet* h) { return UnetEngine::count_launches(h->e.fwd_ops); }
 int ddpm_unet_launch_counts(const ddpm_unet* h, int* fwd, int* bwd, int* pack) {
     if (fwd) *fwd = UnetEngine::count_launches(h->e.fwd_ops);
-    if (bwd) *bwd = UnetEngine::count_launches(h->e.bwd_ops);
+    if (bwd) *bwd = h->e.count_bwd_launches(false, true);     // the default backward (no dx)
     if (pack) *pack = UnetEngine::count_launches(h->e.pack_ops);
     return 0;
 }

@@ -1540,6 +1540,16 @@ __global__ void k_pack_tapco(const float* __restrict__ w /*[CO][C][9]*/, bf16* _
     const int t = i % 9, c = (i / 9) % C, co = i / (9 * C);
     out[(long long)(t * CO + co) * C + c] = __float2bfloat16_rn(w[i]);
 }
+// B operand of in_conv's input gradient on the tensor cores (the mirror of out_conv): in_conv weights w[C][CI][9] ->
+// out[(8 - t)*CI + ci][c] bf16 ([32][C], rows >= 9*CI stay zero).  With the taps flipped, k_out_gather's offsets give the
+// transposed conv dx[b,ci,y,x] = sum_{c,t} dh0[b, y+1-t/3, x+1-t%3, c] * w[c][ci][t].
+__global__ void k_pack_tapflip(const float* __restrict__ w, bf16* __restrict__ out, int C, int CI) {
+    pdl_entry();
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= C * CI * 9) return;
+    const int t = i % 9, ci = (i / 9) % CI, c = i / (9 * CI);
+    out[(long long)((8 - t) * CI + ci) * C + c] = __float2bfloat16_rn(w[i]);
+}
 // transposed pack for the data gradient: out[c][t*CO + co] = w[co][c][t]   ([C][64] bf16, columns >= 9*CO stay zero)
 __global__ void k_pack_tapco_t(const float* __restrict__ w, bf16* __restrict__ out, int CO, int C) {
     pdl_entry();

@@ -20,9 +20,19 @@ struct T4 { long long off = -1; int B = 0, H = 0, W = 0, C = 0;
             long long pix() const { return (long long)B * H * W; } long long numel() const { return pix() * C; } };
 struct Src { T4 t0, t1; bool two = false; int C() const { return t0.C + (two ? t1.C : 0); } };
 enum { OP_TEMB = 1 };
+// Role of a backward op, which decides whether it runs in a given backward variant (ddpm_unet_backward_ex):
+//   DATA   on the path from d_eps to the activation gradients: always runs
+//   PARAM  only feeds the flat gradient buffer (weight gradients, bias column sums, gradient unpacks, the timestep MLP): skipped
+//          when no parameter gradients are asked for
+//   MIXED  produces activation gradients and also writes parameter gradients (GroupNorm dgamma/dbeta and fused column sums, the
+//          gradient-buffer memset): always runs, and drops its flat-buffer writes when no parameter gradients are asked for
+//   DX     the data gradient of in_conv (d_eps -> dx of the network input): runs only when dx is asked for
+enum { ROLE_DATA = 0, ROLE_PARAM = 1, ROLE_MIXED = 2, ROLE_DX = 3 };
 struct Op { std::string name; double flops; std::function<int(cudaStream_t)> run; int launches = 1; bool side = false; int tag = 0;
             int wait_pack = 0;   // forward list: 1 = needs the packed timestep-MLP weights, 2 = first consumer of the packed conv weights
             int chunk = -1;   // >= 0: gradient-chunk boundary of the backward list (see UnetEngine::chunks)
+            int role = ROLE_DATA;
+            bool runs(bool want_dx, bool param_grads) const { return role == ROLE_DX ? want_dx : (role == ROLE_PARAM ? param_grads : true); }
 };
 // A contiguous range [lo, hi) of the flat gradient buffer that is FINAL once `ev` has fired (recorded by the backward pass on the
 // side stream, after the last weight-gradient GEMM / gradient unpack / main-chain reduction that writes into it).  Chunks are
@@ -127,6 +137,13 @@ struct UnetEngine {
     // per-call IO (read by ops at run time)
     const float* x_in = nullptr; const long long* t_in = nullptr; float* eps_out = nullptr;
     unsigned long long drop_seed = 0;
+    // backward variant of the current run (ddpm_unet_backward_ex): the ops run per Op::runs(bwd_dx, bwd_params)
+    bool bwd_params = true, bwd_dx = false;
+    float* dx_dst = nullptr;               // dx f32 [B, Cin, H, W] NCHW of the input-gradient op
+    bool chunks_current = true;            // false after a backward without parameter gradients: no chunk event was recorded
+    float* out_T = nullptr;                // [P][32] tap outputs of the tensor-core out_conv (forward only; reused by the dx op)
+    float* gn_sink = nullptr;              // [2][kGnMaxC] GroupNorm dgamma / dbeta target of a backward without parameter gradients
+                                           // (accumulated into, never read)
     // diffusion-side internal buffers
     size_t xt_off = 0, eps_off = 0, tbuf_off = 0, coefcur_off = 0, counter_off = 0, deps_off = 0;
     size_t bpd_part_off = 0;               // bits/dim per-block partial sums [B * ceil(H*W/256)][2]
@@ -209,10 +226,16 @@ struct UnetEngine {
     GnSrc gsrc(const Src& s) const { GnSrc g; g.x0 = bp(s.t0); g.C0 = s.t0.C; g.x1 = s.two ? bp(s.t1) : nullptr; g.C1 = s.two ? s.t1.C : 0; return g; }
     static Src one(const T4& t) { Src s; s.t0 = t; s.two = false; return s; }
 
+    // role given to backward ops as they are pushed (RoleScope sets it around a builder)
+    int push_role = ROLE_DATA;
+    struct RoleScope { UnetEngine* e; int prev; RoleScope(UnetEngine* e_, int r) : e(e_), prev(e_->push_role) { e->push_role = r; } ~RoleScope() { e->push_role = prev; } };
     void push(std::vector<Op>& L, const std::string& name, double flops, std::function<int(cudaStream_t)> f, int launches = 1, bool side = false) {
-        Op o; o.name = name; o.flops = flops; o.run = std::move(f); o.launches = launches; o.side = side; L.push_back(std::move(o));
+        Op o; o.name = name; o.flops = flops; o.run = std::move(f); o.launches = launches; o.side = side;
+        if (&L == &bwd_ops) o.role = push_role;
+        L.push_back(std::move(o));
     }
     static int count_launches(const std::vector<Op>& L) { int n = 0; for (auto& o : L) n += o.launches; return n; }
+    int count_bwd_launches(bool want_dx, bool param_grads) const { int n = 0; for (auto& o : bwd_ops) if (o.runs(want_dx, param_grads)) n += o.launches; return n; }
     // grad tensor of a forward tensor; `first` tells the producer whether to overwrite (=) or accumulate (+=)
     T4 grad_of(const T4& t, bool* first) {
         auto it = grads.find(t.off);
@@ -397,6 +420,7 @@ struct UnetEngine {
 
     // weight gradient of a conv: dW (OIHW fp32, flat grads) from dy [B,Ho,Wo,Co] and the conv input
     void wgrad_op(const std::string& name, const T4& dy, const Src& in, int ksize, int stride, int map, float* dw, int Co_valid) {
+        RoleScope role(this, ROLE_PARAM);
         const int Cin = in.C(), taps = ksize * ksize, Co = dy.C;
         const long long P = dy.pix();
         const double fl = 2.0 * P * Co_valid * (double)taps * Cin;
@@ -504,7 +528,8 @@ struct UnetEngine {
             return launch_gn_apply(aa, Bn, st); });
         return sv;
     }
-    // dx(in) (=|+=) gn_bwd(dy) + addend ; dgamma/dbeta accumulate into the flat grads
+    // dx(in) (=|+=) gn_bwd(dy) + addend ; dgamma/dbeta (and the optional column sums) accumulate into the flat grads, except in a
+    // backward without parameter gradients, which leaves them out
     void gn_bwd(const std::string& name, const GnSaved& sv, const T4& dy, const bf16* addend,
                 float* cs_per_img = nullptr, int cs_ld = 0, float* cs_total = nullptr, float* cs_total2 = nullptr) {
         const Src& in = sv.in;
@@ -521,11 +546,15 @@ struct UnetEngine {
         static const bool no_dn = getenv("DDPM_GN_NO_DN") != nullptr;
         a.dn_inplace = (sv.silu && !no_dn) ? 1 : 0;
         UnetEngine* self = this;
+        RoleScope role(this, ROLE_MIXED);
         push(bwd_ops, name + ".gn_bwd", 0, [=](cudaStream_t st) {
             GnBwd aa = a; gn_arm_dropout(aa.drop_p, aa.seed, self->drop_seed);
+            if (!self->bwd_params) {          // dgamma / dbeta go to the plan's sink, the column sums are not formed
+                aa.dgamma = self->gn_sink; aa.dbeta = self->gn_sink + kGnMaxC; return launch_gn_bwd(aa, nullptr, 0, nullptr, nullptr, st); }
             return launch_gn_bwd(aa, cs_per_img, cs_ld, cs_total, cs_total2, st); }, 2);
     }
     void colsum_op(const std::string& name, const T4& dy, float* per_img, int ld, float* total, float* total2, int C_valid) {
+        RoleScope role(this, ROLE_PARAM);
         const int HW = dy.H * dy.W, C = dy.C, Bn = dy.B;
         const bf16* p = bp(dy);
         push(bwd_ops, name + ".colsum", 0, [=](cudaStream_t st) { return launch_colsum(p, per_img, ld, total, total2, Bn, HW, C, C_valid, st); }, 1, /*side=*/true);
@@ -612,9 +641,14 @@ struct UnetEngine {
         if (timing_path && !dbg) { tev.resize(L.size() + 1); for (auto& e : tev) cudaEventCreate(&e); cudaEventRecord(tev[0], st); }
         size_t oi = 0; int main_since_fork = 0;
         const bool skip_temb = uniform_t && !temb_uni_ops.empty() && &L == &fwd_ops;
+        const bool is_bwd = &L == &bwd_ops;
         for (auto& o : L) {
             int rc;
             ++oi;
+            if (is_bwd && !o.runs(bwd_dx, bwd_params)) {
+                if (!tev.empty()) cudaEventRecord(tev[oi], st);
+                continue;
+            }
             if (skip_temb && o.tag == OP_TEMB) {
                 if (o.name == "temb.sin") for (auto& u : temb_uni_ops) { rc = u.run(st); if (rc) return fail(-20, "op '%s' failed: %s", u.name.c_str(), cudaGetErrorString((cudaError_t)rc)); }
                 if (!tev.empty()) cudaEventRecord(tev[oi], st);

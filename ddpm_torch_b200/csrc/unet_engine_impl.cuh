@@ -386,7 +386,7 @@ inline int UnetEngine::plan(int B_, int H_, int W_, bool train_, bool dry_) {
     cursor = 0; pack_ops.clear(); fwd_ops.clear(); bwd_ops.clear(); tape.clear(); tape_tag.clear(); cur_tag = "late"; grads.clear(); once_list.clear();
     { std::vector<GradChunk> keep; keep.swap(chunks); for (auto& c : keep) if (c.ev) cudaEventDestroy(c.ev); }
     tp_table_host.clear(); tp_uni_table_host.clear(); fc_table_host.clear(); tpw_table_host.clear(); tpd_table_host.clear(); pack_table_host.clear(); unpack_table_host.clear();
-    layer_counter = 0; fwd_flops = bwd_flops = 0; n_tc_gemms = n_generic = 0; plan_error = 0; gather_fused_tail = false;
+    layer_counter = 0; fwd_flops = bwd_flops = 0; n_tc_gemms = n_generic = 0; plan_error = 0; gather_fused_tail = false; out_T = nullptr;
     const size_t zf_total = zf_cursor, zb_total = zb_cursor;   // sizes learned by the preceding dry pass
     zf_cursor = zb_cursor = 0;
     zero_fwd_bytes = dry ? 0 : zf_total; zero_bwd_bytes = dry ? 0 : zb_total;
@@ -510,8 +510,10 @@ inline int UnetEngine::plan(int B_, int H_, int W_, bool train_, bool dry_) {
         return off;
     };
     if (train) {
-        // adjoint of the embedding MLP; registered first so it runs after every block has deposited its dTP slice
+        // adjoint of the embedding MLP; registered first so it runs after every block has deposited its dTP slice.  The timestep
+        // is an integer input, so all of it only feeds parameter gradients
         tape_push([=]() {
+            RoleScope role(self, ROLE_PARAM);
             const SgemmParams* tw = at<SgemmParams>(tpw_table_off); const SgemmParams* td = at<SgemmParams>(tpd_table_off);
             const dim3 gw((maxc + 63) / 64, (E + 63) / 64, nblocks), gd((E + 63) / 64, (B + 63) / 64, nblocks);
             if (tc_temb) {
@@ -626,6 +628,7 @@ inline int UnetEngine::plan(int B_, int H_, int W_, bool train_, bool dry_) {
             bwd_flops += 2.0 * P * ch * Cin * 9;
             const long long s_c = (long long)Cin * 9;
             static const bool no_tc_in = getenv("DDPM_NO_TC_OUTCONV") != nullptr;
+            RoleScope role(self, ROLE_PARAM);          // the network input's gradient is the dx op at the end of the plan
             if (!no_tc_in && ch % 64 == 0 && tc_ok_geom(H, W) && 9 * Cin <= 64) {
                 // weight gradient on the tensor cores: X = im2col(x) [P][64] bf16, S[ch][64] = dY^T x X (MN-major GEMM, side stream)
                 T4 X = tc_in ? Xcol : newT(B, H, W, 64);
@@ -713,6 +716,7 @@ inline int UnetEngine::plan(int B_, int H_, int W_, bool train_, bool dry_) {
             // tensor-core path: 1x1 GEMM a[P][ch] x W27[32][ch]^T -> fp32 tap outputs T[P][32], then a 9-point gather
             bf16* w27 = at<bf16>(alloc_once_zero((size_t)32 * ch * 2));
             float* T = at<float>(alloc((size_t)B * H * W * 32 * 4));
+            out_T = T;
             const int npk = (Cout * ch * 9 + 255) / 256;
             push(pack_ops, "out_conv.pack27", 0, [=](cudaStream_t st) { launch_k(k_pack_tapco, npk, 256, 0, st, wo, w27, Cout, ch); return (int)cudaGetLastError(); });
             if (train) {
@@ -764,43 +768,57 @@ inline int UnetEngine::plan(int B_, int H_, int W_, bool train_, bool dry_) {
                 const size_t shm2 = (size_t)(ch * Cout * 9 + ch) * 4; const int n2 = grid_for((long long)Bn * Hn * Wn / 2, 128);
                 const long long P = (long long)Bn * Hn * Wn; const int ppb = 256; const int nb = (int)((P + ppb - 1) / ppb);
                 bwd_flops += 2.0 * fl;
+                auto push_bias_grad = [&]() {        // out_conv bias gradient: a parameter-only op of its own
+                    RoleScope role(self, ROLE_PARAM);
+                    push(bwd_ops, "out_conv.2.bias", 0, [=](cudaStream_t st) {
+                        launch_k(k_chansum_nchw, dim3(64, Cout), 256, 0, st, self->deps_src, gb, Bn, Cout, Hn * Wn); return (int)cudaGetLastError(); });
+                };
                 if (tc_out) {
                     // tensor-core backward: E = im2col(d_eps) [P][64] bf16 (shared by both gradients);
                     // d_a = E x W27^T (1x1 conv 64 -> ch), dW = E^T x a (MN-major GEMM on the side stream) -> OIHW
                     T4 E = newT(B, H, W, 64);
                     bf16* Ep = bp(E);
                     const int nim = grid_for((long long)Bn * Hn * Wn);
+                    push_bias_grad();
                     push(bwd_ops, "out_conv.2.im2col", 0, [=](cudaStream_t st) {
                         const float* de = self->deps_src;
-                        launch_k(k_chansum_nchw, dim3(64, Cout), 256, 0, st, de, gb, Bn, Cout, Hn * Wn);
                         switch (Cout) {
                             case 1: launch_k(k_im2col3<1>, nim, 256, 0, st, de, Ep, Bn, Hn, Wn, -1, QsamplePro{nullptr, nullptr, nullptr, nullptr, nullptr}); break;
                             case 2: launch_k(k_im2col3<2>, nim, 256, 0, st, de, Ep, Bn, Hn, Wn, -1, QsamplePro{nullptr, nullptr, nullptr, nullptr, nullptr}); break;
                             default: launch_k(k_im2col3<3>, nim, 256, 0, st, de, Ep, Bn, Hn, Wn, -1, QsamplePro{nullptr, nullptr, nullptr, nullptr, nullptr}); break;
                         }
-                        return (int)cudaGetLastError(); }, 2);
+                        return (int)cudaGetLastError(); });
                     ConvSpec cs; cs.name = "out_conv.2.dgrad"; cs.in = one(E); cs.ksize = 1; cs.wp = w27t; cs.ldw = 64;
                     cs.out = d_a; cs.Co = ch; cs.Ho = H; cs.Wo = W;
                     conv_op(bwd_ops, cs, nullptr);
                     float* S = at<float>(zero_bwd((size_t)64 * ch * 4));
                     wgrad_op("out_conv.2.wgrad", E, one(a_out), 1, 1, MAP_NORMAL, S, 64);
                     const int nun = (Cout * ch * 9 + 255) / 256;
+                    RoleScope role(self, ROLE_PARAM);
                     push(bwd_ops, "out_conv.2.wunpack", 0, [=](cudaStream_t st) { launch_k(k_unpack_tap, nun, 256, 0, st, S, gw, Cout, ch, 0); return (int)cudaGetLastError(); }, 1, true);
-                } else
-                push(bwd_ops, "out_conv.2.bwd", 2.0 * fl, [=](cudaStream_t st) {
-                    const float* de = self->deps_src;
-                    launch_k(k_chansum_nchw, dim3(64, Cout), 256, 0, st, de, gb, Bn, Cout, Hn * Wn);
-                    switch (Cout) {
-                        case 1: launch_k(k_in_conv<1>, n2, 128, shm2, st, de, wt, nullptr, dap, Bn, Hn, Wn, ch, (double*)nullptr, QsamplePro{});
-                                launch_k(k_corr3x3<1>, nb, ch, 0, st, ap, de, gw, 9, (long long)ch * 9, 1, 1, nullptr, Bn, Hn, Wn, ch, ppb); break;
-                        case 2: launch_k(k_in_conv<2>, n2, 128, shm2, st, de, wt, nullptr, dap, Bn, Hn, Wn, ch, (double*)nullptr, QsamplePro{});
-                                launch_k(k_corr3x3<2>, nb, ch, 0, st, ap, de, gw, 9, (long long)ch * 9, 1, 1, nullptr, Bn, Hn, Wn, ch, ppb); break;
-                        case 3: launch_k(k_in_conv<3>, n2, 128, shm2, st, de, wt, nullptr, dap, Bn, Hn, Wn, ch, (double*)nullptr, QsamplePro{});
-                                launch_k(k_corr3x3<3>, nb, ch, 0, st, ap, de, gw, 9, (long long)ch * 9, 1, 1, nullptr, Bn, Hn, Wn, ch, ppb); break;
-                        default: launch_k(k_in_conv<4>, n2, 128, shm2, st, de, wt, nullptr, dap, Bn, Hn, Wn, ch, (double*)nullptr, QsamplePro{});
-                                launch_k(k_corr3x3<4>, nb, ch, 0, st, ap, de, gw, 9, (long long)ch * 9, 1, 1, nullptr, Bn, Hn, Wn, ch, ppb); break;
-                    }
-                    return (int)cudaGetLastError(); }, 3);
+                } else {
+                    // CUDA cores: bias gradient, data gradient (a 3x3 "in_conv" Cout -> ch over d_eps), weight gradient, in that order
+                    push_bias_grad();
+                    push(bwd_ops, "out_conv.2.dgrad", fl, [=](cudaStream_t st) {
+                        const float* de = self->deps_src;
+                        switch (Cout) {
+                            case 1: launch_k(k_in_conv<1>, n2, 128, shm2, st, de, wt, nullptr, dap, Bn, Hn, Wn, ch, (double*)nullptr, QsamplePro{}); break;
+                            case 2: launch_k(k_in_conv<2>, n2, 128, shm2, st, de, wt, nullptr, dap, Bn, Hn, Wn, ch, (double*)nullptr, QsamplePro{}); break;
+                            case 3: launch_k(k_in_conv<3>, n2, 128, shm2, st, de, wt, nullptr, dap, Bn, Hn, Wn, ch, (double*)nullptr, QsamplePro{}); break;
+                            default: launch_k(k_in_conv<4>, n2, 128, shm2, st, de, wt, nullptr, dap, Bn, Hn, Wn, ch, (double*)nullptr, QsamplePro{}); break;
+                        }
+                        return (int)cudaGetLastError(); });
+                    RoleScope role(self, ROLE_PARAM);
+                    push(bwd_ops, "out_conv.2.wgrad", fl, [=](cudaStream_t st) {
+                        const float* de = self->deps_src;
+                        switch (Cout) {
+                            case 1: launch_k(k_corr3x3<1>, nb, ch, 0, st, ap, de, gw, 9, (long long)ch * 9, 1, 1, nullptr, Bn, Hn, Wn, ch, ppb); break;
+                            case 2: launch_k(k_corr3x3<2>, nb, ch, 0, st, ap, de, gw, 9, (long long)ch * 9, 1, 1, nullptr, Bn, Hn, Wn, ch, ppb); break;
+                            case 3: launch_k(k_corr3x3<3>, nb, ch, 0, st, ap, de, gw, 9, (long long)ch * 9, 1, 1, nullptr, Bn, Hn, Wn, ch, ppb); break;
+                            default: launch_k(k_corr3x3<4>, nb, ch, 0, st, ap, de, gw, 9, (long long)ch * 9, 1, 1, nullptr, Bn, Hn, Wn, ch, ppb); break;
+                        }
+                        return (int)cudaGetLastError(); });
+                }
                 gn_bwd("out_conv.0", g, d_a, nullptr);
             });
         }
@@ -808,9 +826,12 @@ inline int UnetEngine::plan(int B_, int H_, int W_, bool train_, bool dry_) {
     // ---- backward list: zero accumulators + flat grads, then the tape in reverse
     if (train) {
         uint8_t* z = ws + zero_bwd_off; const size_t n = zero_bwd_bytes; float* Gp = G; const size_t gbytes = (size_t)flat_elems * 4;
+        {
+        RoleScope role(this, ROLE_MIXED);          // the flat gradient buffer is neither read nor written without parameter gradients
         push(bwd_ops, "zero.bwd", 0, [=](cudaStream_t st) {
             if (n) { const cudaError_t e = cudaMemsetAsync(z, 0, n, st); if (e) return (int)e; }
-            return (int)cudaMemsetAsync(Gp, 0, gbytes, st); }, 0);
+            return self->bwd_params ? (int)cudaMemsetAsync(Gp, 0, gbytes, st) : 0; }, 0);
+        }
         // the tape in reverse; whenever every entry of a level group has run, its slice of the flat gradient buffer is final:
         // groups are merged into chunks of >= 4 M gradients (16 MB) as long as they stay contiguous, and every chunk boundary
         // becomes an op that unpacks the chunk's weight gradients on the side stream and records the chunk's event
@@ -835,7 +856,7 @@ inline int UnetEngine::plan(int B_, int H_, int W_, bool train_, bool dry_) {
             const int idx = (int)chunks.size();
             chunks.push_back(c);
             const int n = c.unpack_hi - c.unpack_lo; const PackEntry* t0 = tab + c.unpack_lo;
-            Op o; o.name = "grad.chunk" + std::to_string(idx); o.flops = 0; o.launches = n > 0 ? 1 : 0; o.chunk = idx;
+            Op o; o.name = "grad.chunk" + std::to_string(idx); o.flops = 0; o.launches = n > 0 ? 1 : 0; o.chunk = idx; o.role = ROLE_PARAM;
             o.run = [=](cudaStream_t st) { if (n > 0) { launch_k(k_pack_table, dim3(128, n), 256, 0, st, t0); return (int)cudaGetLastError(); } return 0; };
             bwd_ops.push_back(std::move(o));
             pend_lo = pend_hi = -1;
@@ -859,6 +880,63 @@ inline int UnetEngine::plan(int B_, int H_, int W_, bool train_, bool dry_) {
     if (!pack_table_host.empty()) {
         const PackEntry* tab = at<PackEntry>(pack_table_off); const int n = (int)pack_table_host.size();
         push(pack_ops, "pack_all", 0, [=](cudaStream_t st) { launch_k(k_pack_table, dim3(128, n), 256, 0, st, tab); return (int)cudaGetLastError(); });
+    }
+    // ---- input gradient (ROLE_DX: only when dx is asked for), dx[b,ci,y,x] = sum_{co,ky,kx} dh0[b, y+1-ky, x+1-kx, co] * W_in[co][ci][ky][kx]:
+    // the mirror of out_conv's forward (NHWC bf16 [P][ch] -> narrow NCHW fp32), on the same two routes with the same selection rule.
+    //   tensor cores: k_pack_tapflip -> Wdx[32][ch] bf16 (taps flipped); dh0 x Wdx^T -> T[P][32] fp32 (out_conv's KK GEMM); then
+    //                 k_out_gather<Cin> without bias: with the taps flipped, the gather's offsets give the transposed conv
+    //   CUDA cores:   k_flip_transpose_w -> [Cin][ch][9] fp32; k_out_conv<Cin> over dh0 with a zero bias
+    // The ops come after the whole tape, so every contribution to dh0 (the first down block's norm1 and residual, the last up block's
+    // skip concat) has landed on the main stream; the weights are packed from the fp32 masters by the dx pass itself.  Its buffers sit
+    // behind everything else, so the default plan's workspace layout, pack table and launch list are those of a plan without it.
+    // Not counted in the plan's FLOPs or tensor-core ops, which describe the default backward.
+    if (train) {
+        gn_sink = at<float>(alloc_once_zero((size_t)2 * kGnMaxC * 4));
+        RoleScope role(this, ROLE_DX);
+        const T4 dh0 = grad_of(h0, nullptr);
+        const bf16* d = bp(dh0); const float* wi = PP("in_conv.weight");
+        const int Bn = B, Hn = H, Wn = W; const long long P = (long long)B * H * W;
+        const double fl = 2.0 * P * ch * Cin * 9;
+        const int nblk = grid_for(P), npk = (ch * Cin * 9 + 255) / 256;
+        const bool tc_dx = !getenv("DDPM_NO_TC_OUTCONV") && ch % 64 == 0 && tc_ok_geom(H, W) && 9 * Cin <= 32;
+        if (tc_dx) {
+            bf16* wdx = at<bf16>(alloc_once_zero((size_t)32 * ch * 2));
+            float* T = out_T ? out_T : at<float>(alloc((size_t)P * 32 * 4));     // out_conv's forward scratch is dead by now
+            push(bwd_ops, "in_conv.dx.pack", 0, [=](cudaStream_t st) { launch_k(k_pack_tapflip, npk, 256, 0, st, wi, wdx, ch, Cin); return (int)cudaGetLastError(); });
+            ddpm_gemm_desc g; memset(&g, 0, sizeof g);
+            g.mode = GEMM_KK; g.M = (int)P; g.N = 32; g.block_n = 64; g.W = W; g.H = H; g.NB = B;
+            g.a_ptr[0] = d; g.a_C[0] = ch; g.a_ld[0] = ch;
+            g.nseg = 1; g.seg_map[0] = 0; g.seg_taps[0] = 1; g.seg_kchunks[0] = ch / 64; g.seg_cbase[0] = 0;
+            g.b_ptr = wdx; g.b_K = ch; g.b_rows = 32; g.b_batch = 1; g.b_ld = ch; g.b_bs = 0;
+            g.out = T; g.ldo = 32; g.alpha = 1.f; g.grid_z = 1; g.flags = EPI_OUT_F32;
+            if (dry) push(bwd_ops, "in_conv.dx", fl, [](cudaStream_t) { return 0; });
+            else {
+                GemmLaunch gl; const int rc = build_gemm(g, gl);
+                if (rc) return rc;
+                push(bwd_ops, "in_conv.dx", fl, [gl](cudaStream_t st) { return launch_gemm(gl, st); });
+            }
+            push(bwd_ops, "in_conv.dx.gather", 0, [=](cudaStream_t st) {
+                const PsampleEpi no_ps{nullptr, nullptr, nullptr, 0, nullptr}; const BpdEpi no_bpd{};
+                switch (Cin) {
+                    case 1: launch_k(k_out_gather<1>, nblk, 256, 0, st, (const float*)T, (const float*)nullptr, self->dx_dst, Bn, Hn, Wn, no_ps, no_bpd); break;
+                    case 2: launch_k(k_out_gather<2>, nblk, 256, 0, st, (const float*)T, (const float*)nullptr, self->dx_dst, Bn, Hn, Wn, no_ps, no_bpd); break;
+                    default: launch_k(k_out_gather<3>, nblk, 256, 0, st, (const float*)T, (const float*)nullptr, self->dx_dst, Bn, Hn, Wn, no_ps, no_bpd); break;
+                }
+                return (int)cudaGetLastError(); });
+        } else {
+            float* wt = at<float>(alloc((size_t)Cin * ch * 9 * 4));
+            const float* zb = at<float>(alloc_once_zero(64));
+            push(bwd_ops, "in_conv.dx.pack", 0, [=](cudaStream_t st) { launch_k(k_flip_transpose_w, npk, 256, 0, st, wi, wt, ch, Cin); return (int)cudaGetLastError(); });
+            const size_t shm = (size_t)9 * Cin * ch * 4;
+            push(bwd_ops, "in_conv.dx", fl, [=](cudaStream_t st) {
+                switch (Cin) {
+                    case 1: launch_k(k_out_conv<1>, nblk, 256, shm, st, d, (const float*)wt, zb, self->dx_dst, Bn, Hn, Wn, ch); break;
+                    case 2: launch_k(k_out_conv<2>, nblk, 256, shm, st, d, (const float*)wt, zb, self->dx_dst, Bn, Hn, Wn, ch); break;
+                    case 3: launch_k(k_out_conv<3>, nblk, 256, shm, st, d, (const float*)wt, zb, self->dx_dst, Bn, Hn, Wn, ch); break;
+                    default: launch_k(k_out_conv<4>, nblk, 256, shm, st, d, (const float*)wt, zb, self->dx_dst, Bn, Hn, Wn, ch); break;
+                }
+                return (int)cudaGetLastError(); });
+        }
     }
     if (plan_error) return plan_error;
     return 0;

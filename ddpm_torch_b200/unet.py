@@ -259,7 +259,8 @@ class UNet(nn.Module):
         assert Cc == self.in_channels
         x = x.contiguous().float()
         t = t.contiguous().to(torch.int64)
-        need_grad = torch.is_grad_enabled() and any(p.requires_grad for p in self._params)
+        # autograd path when anything needs a gradient: the parameters (training), the input (guidance, saliency), or both
+        need_grad = torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in self._params))
         if need_grad:
             return _UNetFn.apply(self, x, t, *self._params)
         return self._forward_nograd(x, t)
@@ -279,7 +280,9 @@ class UNet(nn.Module):
 
 
 class _UNetFn(torch.autograd.Function):
-    """Autograd bridge: parameter gradients come back as views of one freshly cloned flat buffer."""
+    """Autograd bridge: parameter gradients come back as views of one freshly cloned flat buffer, the input gradient as an
+    NCHW fp32 tensor.  Only what autograd asks for is computed: a frozen model's backward runs no weight-gradient op and
+    leaves the flat gradient buffer (and any accumulation in progress in it) untouched."""
 
     @staticmethod
     def forward(ctx, model, x, t, *params):
@@ -291,13 +294,20 @@ class _UNetFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, grad_out):
         model = ctx.model
+        want_dx = ctx.needs_input_grad[1]
+        want_params = any(ctx.needs_input_grad[3:])
+        if not (want_dx or want_params):
+            return (None,) * (3 + len(ctx.needs_input_grad[3:]))
         g = grad_out.contiguous().float()
         dev = model._flat.device
-        model._before_backward()
+        dx = torch.empty(ctx.saved_tensors[0].shape, dtype=torch.float32, device=dev) if want_dx else None
+        if want_params:
+            model._before_backward()
         with torch.cuda.device(dev):
-            _lib.check(_lib.lib().ddpm_unet_backward(model._h, g.data_ptr(), _lib.stream_ptr(dev)), "unet_backward")
-        flat = model._grads.clone()
-        return (None, None, None, *model.grad_views(flat))
+            _lib.check(_lib.lib().ddpm_unet_backward_ex(model._h, g.data_ptr(), dx.data_ptr() if want_dx else None,
+                                                        int(want_params), _lib.stream_ptr(dev)), "unet_backward")
+        grads = model.grad_views(model._grads.clone()) if want_params else [None] * len(model._params)
+        return (None, dx, None, *grads)
 
 
 class ModelWrapper(nn.Module):

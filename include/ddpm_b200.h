@@ -191,8 +191,22 @@ int ddpm_unet_plan(ddpm_unet* h, int B, int H, int W, int training, float* param
 int ddpm_unet_repack(ddpm_unet* h, void* stream);
 /* eps = UNet(x, t):  x f32[B,Cin,H,W] NCHW, t i64[B], eps f32[B,Cout,H,W]   (unet.py:205-233) */
 int ddpm_unet_forward(ddpm_unet* h, const float* x, const int64_t* t, float* eps, uint64_t dropout_seed, void* stream);
-/* Backward of the last forward: d_eps f32[B,Cout,H,W] -> flat grads (zeroed then written). x,t must be unchanged. */
+/* Backward of the last forward: d_eps f32[B,Cout,H,W] -> flat grads (zeroed then written). x,t must be unchanged.
+ * Same as ddpm_unet_backward_ex(h, d_eps, NULL, 1, stream). */
 int ddpm_unet_backward(ddpm_unet* h, const float* d_eps, void* stream);
+/* Backward of the last forward with a choice of outputs (autograd of unet.py:205-233 with respect to x and/or the parameters):
+ *  dx           f32[B,Cin,H,W] NCHW <- d(eps . d_eps)/dx, the gradient with respect to the network input (guided sampling,
+ *               inverse problems, saliency); NULL = not computed.
+ *  param_grads  1: the flat gradients are zeroed and then written, as ddpm_unet_backward does;
+ *               0: no weight-gradient op runs and the flat gradient buffer is neither read nor written (a frozen model whose
+ *               caller may be accumulating gradients of another backward in it).  No gradient-chunk event is recorded:
+ *               ddpm_unet_wait_grad_chunk then fails until the next backward with parameter gradients.
+ * Refused before any launch without a training plan, when param_grads is not 0 or 1, or when param_grads = 0 and dx = NULL.
+ * CUDA-graph capturable. */
+int ddpm_unet_backward_ex(ddpm_unet* h, const float* d_eps, float* dx, int param_grads, void* stream);
+/* Kernel launches of one backward of the compiled (or dry-planned) training plan in the variant (want_dx, param_grads), flags
+ * 0 or 1 and not both 0 (memsets not counted); (0, 1) is the backward of ddpm_unet_launch_counts.  < 0 on error. */
+int ddpm_unet_backward_launches(const ddpm_unet* h, int want_dx, int param_grads);
 /* Fused training forward (diffusion.py:217-243, mse/eps branch): x_t = q_sample(x0,t,noise) with the fp32 tables
  * tab_sqrt_ab / tab_sqrt_1mab [T]; eps = UNet(x_t,t); losses[b] = mean((noise-eps)^2).
  * Needs out_channels == in_channels (fails before any launch otherwise), as do the sampler steps below. */
