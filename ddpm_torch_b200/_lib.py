@@ -74,6 +74,21 @@ class GnBwdDesc(C.Structure):
     ]
 
 
+class AttnDesc(C.Structure):
+    _fields_ = [
+        ("route", C.c_int), ("NB", C.c_int), ("T", C.c_int), ("C", C.c_int),
+        ("qkv", C.c_void_p), ("out", C.c_void_p), ("probs", C.c_void_p), ("scratch", C.c_void_p),
+    ]
+
+
+class AttnBwdDesc(C.Structure):
+    _fields_ = [
+        ("route", C.c_int), ("NB", C.c_int), ("T", C.c_int), ("C", C.c_int),
+        ("qkv", C.c_void_p), ("d_out", C.c_void_p), ("probs", C.c_void_p),
+        ("d_qkv", C.c_void_p), ("d_scores", C.c_void_p), ("scratch", C.c_void_p),
+    ]
+
+
 class UnetCfg(C.Structure):
     _fields_ = [("in_channels", C.c_int), ("hid_channels", C.c_int), ("out_channels", C.c_int),
                 ("levels", C.c_int), ("ch_mult", C.c_int * 8), ("num_res_blocks", C.c_int), ("attn", C.c_int * 8),
@@ -107,6 +122,9 @@ def lib():
             "ddpm_conv_halo_run": ([C.POINTER(HaloDesc), vp], i32),
             "ddpm_attn_fused_run": ([vp, vp, vp, i32, i32, i32, vp], i32),
             "ddpm_attn_fused_bwd_run": ([vp, vp, vp, vp, vp, i32, i32, i32, vp], i32),
+            "ddpm_attention_fwd_run": ([C.POINTER(AttnDesc), vp], i32),
+            "ddpm_attention_bwd_run": ([C.POINTER(AttnBwdDesc), vp], i32),
+            "ddpm_attn_scratch_bytes": ([i32, i32, i32, i32, i32], i64),
             "ddpm_gn_scratch_bytes": ([i32, i32], i64),
             "ddpm_groupnorm_fwd_run": ([C.POINTER(GnDesc), vp], i32),
             "ddpm_groupnorm_bwd_run": ([C.POINTER(GnBwdDesc), vp], i32),
@@ -151,6 +169,7 @@ def lib():
 
 
 EXPORTS = ["ddpm_last_error", "ddpm_runtime_check", "ddpm_device_error_flag", "ddpm_gemm_run", "ddpm_conv_halo_run", "ddpm_attn_fused_run", "ddpm_attn_fused_bwd_run",
+           "ddpm_attention_fwd_run", "ddpm_attention_bwd_run", "ddpm_attn_scratch_bytes",
            "ddpm_gn_scratch_bytes", "ddpm_groupnorm_fwd_run", "ddpm_groupnorm_bwd_run", "ddpm_colsum_run",
            "ddpm_unet_create", "ddpm_unet_create_ex", "ddpm_unet_destroy", "ddpm_unet_num_params", "ddpm_unet_param_info",
            "ddpm_unet_flat_elems", "ddpm_unet_workspace_bytes", "ddpm_unet_plan", "ddpm_unet_repack",

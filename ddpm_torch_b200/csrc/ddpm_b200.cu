@@ -170,6 +170,83 @@ int ddpm_colsum_run(const void* dy, float* per_img, int ld, float* total, float*
     return rc ? fail(-20, "%s: %s", fn, cudaGetErrorString((cudaError_t)rc)) : 0;
 }
 
+// ------------------------------------------------------------------------------------------------ attention core
+// scratch layout.  route 3 forward: S f32 [NB][T][T].  route 3 backward: dP f32 [NB][T][T] | dS bf16 [NB][T][T].  route 1 backward:
+// dS bf16 [NB][T][T].  The dS area is used only when the caller passes no d_scores.
+static size_t attn_scratch(int route, int NB, int T, int backward) {
+    const size_t tt = (size_t)NB * T * T;
+    if (route == ATTN_ROUTE_PRODUCTS) return gn_align(tt * 4) + (backward ? gn_align(tt * 2) : 0);
+    if (route == ATTN_ROUTE_FUSED && backward) return gn_align(tt * 2);
+    return 0;
+}
+static int attn_check(const char* fn, int route, int NB, int T, int C) {
+    if (route < 1 || route > 3) return fail(-43, "%s: route must be 1 (fused), 2 (t16) or 3 (products + row softmax)", fn);
+    if (NB < 1 || T < 1 || C < 1) return fail(-43, "%s: need NB >= 1, T >= 1 and C >= 1", fn);
+    if (NB > 65535) return fail(-43, "%s: NB = %d exceeds 65535 (one grid z slice per image)", fn, NB);
+    if (C % 8) return fail(-43, "%s: C must be a multiple of 8 (got %d)", fn, C);
+    if (route == ATTN_ROUTE_FUSED && !attn_fused_eligible(T, C))
+        return fail(-43, "%s: route 1 (fused) needs T = 256 and C = 256 (got T = %d, C = %d)", fn, T, C);
+    if (route == ATTN_ROUTE_T16 && !attn16_eligible(T, C))
+        return fail(-43, "%s: route 2 (t16) needs T = 16 and C in {128, 256, 512} (got T = %d, C = %d)", fn, T, C);
+    return 0;
+}
+static int attn_run(const char* fn, const AttnSteps& steps, void* stream) {
+    for (const AttnStep& s : steps) {
+        const int rc = s.run(static_cast<cudaStream_t>(stream));
+        if (rc) return fail(-20, "%s: launch '%s' failed: %s", fn, s.name.c_str(), cudaGetErrorString((cudaError_t)rc));
+    }
+    return 0;
+}
+
+long long ddpm_attn_scratch_bytes(int route, int NB, int T, int C, int backward) {
+    const char* fn = "ddpm_attn_scratch_bytes";
+    const int rc = attn_check(fn, route, NB, T, C);
+    if (rc) return rc;
+    if (backward != 0 && backward != 1) return fail(-43, "%s: backward must be 0 or 1 (got %d)", fn, backward);
+    return (long long)attn_scratch(route, NB, T, backward);
+}
+
+int ddpm_attention_fwd_run(const ddpm_attn_desc* d, void* stream) {
+    const char* fn = "ddpm_attention_fwd_run";
+    if (!d) return fail(-43, "%s: null descriptor", fn);
+    int rc = attn_check(fn, d->route, d->NB, d->T, d->C);
+    if (rc) return rc;
+    if (!d->qkv || !d->out) return fail(-43, "%s: null buffer (qkv and out are required)", fn);
+    if (d->route == ATTN_ROUTE_PRODUCTS && !d->probs) return fail(-43, "%s: route 3 writes the probabilities: probs is required", fn);
+    if (attn_scratch(d->route, d->NB, d->T, 0) && !d->scratch)
+        return fail(-43, "%s: route %d needs a scratch area of ddpm_attn_scratch_bytes bytes", fn, d->route);
+    if (misaligned16(d->qkv) || misaligned16(d->out) || misaligned16(d->probs) || misaligned16(d->scratch))
+        return fail(-43, "%s: qkv, out, probs and scratch must be 16-byte aligned", fn);
+    AttnSteps steps;
+    rc = attn_fwd_steps(steps, d->route, static_cast<const bf16*>(d->qkv), static_cast<bf16*>(d->out), static_cast<bf16*>(d->probs),
+                        static_cast<float*>(d->scratch), d->NB, d->T, d->C, false);
+    return rc ? rc : attn_run(fn, steps, stream);
+}
+
+int ddpm_attention_bwd_run(const ddpm_attn_bwd_desc* d, void* stream) {
+    const char* fn = "ddpm_attention_bwd_run";
+    if (!d) return fail(-43, "%s: null descriptor", fn);
+    int rc = attn_check(fn, d->route, d->NB, d->T, d->C);
+    if (rc) return rc;
+    if (!d->qkv || !d->d_out || !d->d_qkv) return fail(-43, "%s: null buffer (qkv, d_out and d_qkv are required)", fn);
+    if (!d->probs) return fail(-43, "%s: the backward reads the probabilities its forward wrote: probs is required", fn);
+    const size_t sb = attn_scratch(d->route, d->NB, d->T, 1);
+    if (sb && !d->scratch) return fail(-43, "%s: route %d needs a scratch area of ddpm_attn_scratch_bytes bytes", fn, d->route);
+    if (misaligned16(d->qkv) || misaligned16(d->d_out) || misaligned16(d->probs) || misaligned16(d->d_qkv) || misaligned16(d->d_scores) ||
+        misaligned16(d->scratch))
+        return fail(-43, "%s: qkv, d_out, probs, d_qkv, d_scores and scratch must be 16-byte aligned", fn);
+    uint8_t* s = static_cast<uint8_t*>(d->scratch);
+    float* dP = d->route == ATTN_ROUTE_PRODUCTS ? reinterpret_cast<float*>(s) : nullptr;
+    bf16* dS = nullptr;
+    if (d->route != ATTN_ROUTE_T16)
+        dS = d->d_scores ? static_cast<bf16*>(d->d_scores)
+                         : reinterpret_cast<bf16*>(s + (d->route == ATTN_ROUTE_PRODUCTS ? gn_align((size_t)d->NB * d->T * d->T * 4) : 0));
+    AttnSteps steps;
+    rc = attn_bwd_steps(steps, d->route, static_cast<const bf16*>(d->qkv), static_cast<const bf16*>(d->d_out), static_cast<const bf16*>(d->probs),
+                        dP, dS, static_cast<bf16*>(d->d_qkv), d->NB, d->T, d->C, false);
+    return rc ? rc : attn_run(fn, steps, stream);
+}
+
 // ------------------------------------------------------------------------------------------------ UNet engine
 int ddpm_unet_create(const ddpm_unet_cfg* cfg, ddpm_unet** out) { return ddpm_unet_create_ex(cfg, 1, out); }
 int ddpm_unet_create_ex(const ddpm_unet_cfg* cfg, int resample_with_conv, ddpm_unet** out) {

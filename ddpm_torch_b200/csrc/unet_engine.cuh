@@ -105,6 +105,157 @@ static inline int launch_colsum(const bf16* dy, float* per_img, int ld, float* t
     return (int)cudaGetLastError();
 }
 
+// ------------------------------------------------------------------ attention core launches
+// softmax(Q K^T / sqrt(C)) V of AttentionBlock (unet.py:43-51) and its backward, with qkv bf16 [NB][T][3C].  Shared by the engine's
+// plans (attn_block) and the attention operators of the C ABI: a route is built as a list of launch steps, which the engine pushes
+// as ops named <block> + step.name and the operators run in order, so both launch the same kernels with the same grids.
+//   1 fused     T = 256, C = 256: attn_kernel<false> (attn_fused.cuh); backward attn_kernel<true> + the dV / dK products
+//   2 t16       T = 16, C in {128, 256, 512}: k_attn16_fwd / k_attn16_bwd, one CTA per image
+//   3 products  Q.K^T -> k_softmax_rows -> P.V; backward dP, dV, k_softmax_bwd, dQ, dK.  The products run on the GEMM engine when
+//               attn_bmm_tc(T, C), on CUDA cores (k_sgemm) otherwise
+enum { ATTN_ROUTE_FUSED = 1, ATTN_ROUTE_T16 = 2, ATTN_ROUTE_PRODUCTS = 3 };
+enum { ATTN_STEP_AUX = 0, ATTN_STEP_TC = 1, ATTN_STEP_SIMT = 2 };   // what a step counts as in the plan statistics
+struct AttnStep { std::string name; double flops; int kind; std::function<int(cudaStream_t)> run; };
+using AttnSteps = std::vector<AttnStep>;
+
+// the products of route 3 take the GEMM engine for a power-of-two T that is a multiple of 128 and C % 64 == 0
+inline bool attn_bmm_tc(int T, int Cc) { return (T % 128 == 0) && (Cc % 64 == 0) && ((T & (T - 1)) == 0); }
+
+// k_attn16_* need attn16_smem(512, .) bytes of dynamic shared memory at C = 512: raise the limit once per device.  The engine calls
+// this at plan time, so that no launch of a plan (which may be under graph capture) has to
+inline int attn16_prepare() {
+    static unsigned done = 0;
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return (int)e;
+    if (dev < 32 && ((done >> dev) & 1u)) return 0;
+    e = cudaFuncSetAttribute(k_attn16_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn16_smem(512, false));
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_attn16_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn16_smem(512, true));
+    if (e != cudaSuccess) return (int)e;
+    if (dev < 32) done |= 1u << dev;
+    return 0;
+}
+static inline int launch_attn16_fwd(const bf16* qkv, bf16* O, bf16* P, int NB, int C, float scale, cudaStream_t st) {
+    const int rc = attn16_prepare(); if (rc) return rc;
+    launch_k(k_attn16_fwd, NB, 256, attn16_smem(C, false), st, qkv, O, P, C, scale);
+    return (int)cudaGetLastError();
+}
+static inline int launch_attn16_bwd(const bf16* qkv, const bf16* dO, const bf16* P, bf16* dqkv, int NB, int C, float scale, cudaStream_t st) {
+    const int rc = attn16_prepare(); if (rc) return rc;
+    launch_k(k_attn16_bwd, NB, 256, attn16_smem(C, true), st, qkv, dO, P, dqkv, C, scale);
+    return (int)cudaGetLastError();
+}
+// one warp per row of [rows][T]
+static inline int launch_softmax_rows(const float* S, bf16* P, long long rows, int T, cudaStream_t st) {
+    launch_k(k_softmax_rows, (int)((rows + 7) / 8), 256, 0, st, S, P, rows, T);
+    return (int)cudaGetLastError();
+}
+static inline int launch_softmax_bwd(const bf16* P, const float* dP, bf16* dS, long long rows, int T, float scale, cudaStream_t st) {
+    launch_k(k_softmax_bwd, (int)((rows + 7) / 8), 256, 0, st, P, dP, dS, rows, T, scale);
+    return (int)cudaGetLastError();
+}
+
+// Batched matmuls of the attention block (unet.py:43-51) and their adjoints.
+//   form 0 (NT): C[b][i][j] = alpha * sum_c A[b][i][c] * B[b][j][c]     M=i, N=j, K=c
+//   form 1 (NN): C[b][i][c] = sum_j A[b][i][j] * B[b][j][c]             M=i, N=c, K=j
+//   form 2 (TN): C[b][j][c] = sum_i A[b][i][j] * B[b][i][c]             M=j, N=c, K=i
+// A, B bf16 with row strides lda/ldb and per-batch strides = rows*ld; C bf16 or fp32.  A dry plan builds no tensor maps: its
+// tensor-core step does nothing.
+inline int attn_bmm(AttnSteps& S, const std::string& name, int form, const bf16* A, long long lda, long long sa,
+                    const bf16* Bp, long long ldb, long long sb, void* C, long long ldc, long long sc, bool c_f32,
+                    int nb, int T, int Cc, float alpha, bool dry) {
+    // all attention products here are T x T x Cc shaped
+    const int M = T, N = (form == 0) ? T : Cc, K = (form == 0) ? Cc : T;
+    const double fl = 2.0 * nb * (double)M * N * K;
+    if (attn_bmm_tc(T, Cc)) {
+        ddpm_gemm_desc d; memset(&d, 0, sizeof d);
+        d.M = M; d.N = N; d.W = T; d.H = 1; d.NB = nb; d.alpha = alpha; d.grid_z = nb;
+        d.out = C; d.ldo = (int)ldc; d.out_z_stride = sc; d.flags = c_f32 ? EPI_OUT_F32 : 0;
+        d.a_ptr[0] = A; d.a_ld[0] = lda;
+        if (form == 0) {
+            d.mode = GEMM_KK; d.a_C[0] = K; d.nseg = 1; d.seg_map[0] = 0; d.seg_taps[0] = 1; d.seg_kchunks[0] = K / 64; d.seg_cbase[0] = 0;
+            d.b_ptr = Bp; d.b_K = K; d.b_rows = N; d.b_batch = nb; d.b_ld = ldb; d.b_bs = sb; d.a_z_n = 1; d.b_z = 1;
+        } else if (form == 1) {
+            d.mode = GEMM_KMN; d.a_C[0] = K; d.b_ptr = Bp; d.b_K = N; d.b_ld = ldb; d.kblocks = K / 64; d.a_z_n = 1;
+        } else {
+            d.mode = GEMM_MNMN; d.a_C[0] = M; d.b_ptr = Bp; d.b_K = N; d.b_ld = ldb; d.taps = 1; d.splits = 1; d.kblocks = K / 64;
+        }
+        if (dry) { S.push_back({name, fl, ATTN_STEP_TC, [](cudaStream_t) { return 0; }}); return 0; }
+        GemmLaunch g; const int rc = build_gemm(d, g);
+        if (rc) return rc;
+        S.push_back({name, fl, ATTN_STEP_TC, [g](cudaStream_t st) { return launch_gemm(g, st); }});
+        return 0;
+    }
+    SgemmParams p; memset(&p, 0, sizeof p);
+    p.A = A; p.B = Bp; p.C = C; p.M = M; p.N = N; p.K = K; p.alpha = alpha;
+    p.sa_z = sa; p.sb_z = sb; p.sc_z = sc; p.sc_m = ldc; p.sc_n = 1;
+    if (form == 0) { p.sa_m = lda; p.sa_k = 1; p.sb_k = 1; p.sb_n = ldb; }
+    else if (form == 1) { p.sa_m = lda; p.sa_k = 1; p.sb_k = ldb; p.sb_n = 1; }
+    else { p.sa_m = 1; p.sa_k = lda; p.sb_k = ldb; p.sb_n = 1; }
+    const dim3 grid((N + 63) / 64, (M + 63) / 64, nb);
+    if (c_f32) S.push_back({name + "[simt]", fl, ATTN_STEP_SIMT, [p, grid](cudaStream_t st) { launch_k(k_sgemm<bf16, bf16, float>, grid, 256, 0, st, p); return (int)cudaGetLastError(); }});
+    else       S.push_back({name + "[simt]", fl, ATTN_STEP_SIMT, [p, grid](cudaStream_t st) { launch_k(k_sgemm<bf16, bf16, bf16>, grid, 256, 0, st, p); return (int)cudaGetLastError(); }});
+    return 0;
+}
+
+// forward of `route`: O bf16 [NB][T][C]; P bf16 [NB][T][T] (routes 1 and 2: written when not null; route 3: always);
+// S fp32 [NB][T][T] (route 3 only)
+inline int attn_fwd_steps(AttnSteps& out, int route, const bf16* qkv, bf16* O, bf16* P, float* S, int NB, int T, int C, bool dry) {
+    const float scale = 1.f / sqrtf((float)C);
+    const long long ldq = 3 * C, sq = (long long)T * 3 * C, tt = (long long)T * T;
+    const double fl = 4.0 * NB * (double)T * T * C;
+    if (route == ATTN_ROUTE_FUSED) {
+        // Q.K^T -> softmax -> P.V in ONE kernel, S and O in registers, P in shared memory (attn_fused.cuh)
+        if (dry) { out.push_back({".attn[fused]", fl, ATTN_STEP_TC, [](cudaStream_t) { return 0; }}); return 0; }
+        AttnLaunch g; const int rc = build_attn(qkv, O, NB, T, C, g, P);
+        if (rc) return rc;
+        out.push_back({".attn[fused]", fl, ATTN_STEP_TC, [g](cudaStream_t st) { return launch_attn(g, st); }});
+        return 0;
+    }
+    if (route == ATTN_ROUTE_T16) {
+        // 4x4 level: one CTA per image does scores, softmax and P.V
+        out.push_back({".attn[t16]", fl, ATTN_STEP_SIMT, [=](cudaStream_t st) { return launch_attn16_fwd(qkv, O, P, NB, C, scale, st); }});
+        return 0;
+    }
+    int rc = attn_bmm(out, ".qk", 0, qkv, ldq, sq, qkv + C, ldq, sq, S, T, tt, true, NB, T, C, scale, dry);
+    if (rc) return rc;
+    const long long rows = (long long)NB * T;
+    out.push_back({".softmax", 0, ATTN_STEP_AUX, [=](cudaStream_t st) { return launch_softmax_rows(S, P, rows, T, st); }});
+    return attn_bmm(out, ".pv", 1, P, T, tt, qkv + 2 * C, ldq, sq, O, C, (long long)T * C, false, NB, T, C, 1.f, dry);
+}
+
+// backward of `route` from the P its forward wrote: dO bf16 [NB][T][C] -> all three thirds of dqkv bf16 [NB][T][3C].
+// dS bf16 [NB][T][T] (routes 1 and 3) and dP fp32 [NB][T][T] (route 3) are intermediates the route materialises
+inline int attn_bwd_steps(AttnSteps& out, int route, const bf16* qkv, const bf16* dO, const bf16* P, float* dP, bf16* dS, bf16* dqkv,
+                          int NB, int T, int C, bool dry) {
+    const float scale = 1.f / sqrtf((float)C);
+    const long long ldq = 3 * C, sq = (long long)T * 3 * C, tt = (long long)T * T, so = (long long)T * C;
+    if (route == ATTN_ROUTE_T16) {
+        const double fl = 8.0 * NB * (double)T * T * C;
+        out.push_back({".attn_bwd[t16]", fl, ATTN_STEP_SIMT, [=](cudaStream_t st) { return launch_attn16_bwd(qkv, dO, P, dqkv, NB, C, scale, st); }});
+        return 0;
+    }
+    int rc;
+    if (route == ATTN_ROUTE_FUSED) {
+        // dP -> softmax backward -> dQ in one launch (attn_kernel<true>); dK and dV read dS / P back as GEMM operands
+        const double fl = 4.0 * NB * (double)T * T * C;
+        if (dry) out.push_back({".attn_bwd[fused]", fl, ATTN_STEP_TC, [](cudaStream_t) { return 0; }});
+        else {
+            AttnLaunch g;
+            if ((rc = build_attn_bwd(qkv, dO, P, dS, dqkv, NB, T, C, g))) return rc;
+            out.push_back({".attn_bwd[fused]", fl, ATTN_STEP_TC, [g](cudaStream_t st) { return launch_attn_bwd(g, st); }});
+        }
+        if ((rc = attn_bmm(out, ".dV", 2, P, T, tt, dO, C, so, dqkv + 2 * C, ldq, sq, false, NB, T, C, 1.f, dry))) return rc;
+        return attn_bmm(out, ".dK", 2, dS, T, tt, qkv, ldq, sq, dqkv + C, ldq, sq, false, NB, T, C, 1.f, dry);
+    }
+    if ((rc = attn_bmm(out, ".dP", 0, dO, C, so, qkv + 2 * C, ldq, sq, dP, T, tt, true, NB, T, C, 1.f, dry))) return rc;
+    if ((rc = attn_bmm(out, ".dV", 2, P, T, tt, dO, C, so, dqkv + 2 * C, ldq, sq, false, NB, T, C, 1.f, dry))) return rc;
+    const long long rows = (long long)NB * T;
+    out.push_back({".softmax_bwd", 0, ATTN_STEP_AUX, [=](cudaStream_t st) { return launch_softmax_bwd(P, dP, dS, rows, T, scale, st); }});
+    if ((rc = attn_bmm(out, ".dQ", 1, dS, T, tt, qkv + C, ldq, sq, dqkv, ldq, sq, false, NB, T, C, 1.f, dry))) return rc;
+    return attn_bmm(out, ".dK", 2, dS, T, tt, qkv, ldq, sq, dqkv + C, ldq, sq, false, NB, T, C, 1.f, dry);
+}
+
 struct UnetEngine {
     ddpm_unet_cfg cfg;
     bool resample_with_conv = true;       // false: AvgPool2d(2) / bare nearest x2 instead of the resample convs (unet.py:164-170,199-202)
@@ -600,8 +751,7 @@ struct UnetEngine {
     T4 up_conv(const std::string& p, const T4& x);
     T4 down_pool(const std::string& p, const T4& x);
     T4 up_nearest(const std::string& p, const T4& x);
-    void bmm(std::vector<Op>& L, const std::string& name, int form, const bf16* A, long long lda, long long sa, const bf16* Bp, long long ldb, long long sb,
-             void* C, long long ldc, long long sc, bool c_f32, int nb, int T, int Cc, float alpha, double* fl_acc);
+    void push_attn_steps(std::vector<Op>& L, const std::string& p, const AttnSteps& steps, double& flops_acc);
     int plan(int B_, int H_, int W_, bool train_, bool dry_);
     int build();
     // Ops flagged `side` (bias-gradient column sums, gradient unpacks: small, memory-bound, nothing downstream needs them

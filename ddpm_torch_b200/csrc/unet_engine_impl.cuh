@@ -1,53 +1,18 @@
-// UNet engine, part 2: block builders (forward ops + adjoint tape), batched attention matmuls, plan().
+// UNet engine, part 2: block builders (forward ops + adjoint tape), plan().
 #pragma once
 #include <cmath>
 #include "unet_engine.cuh"
 
 namespace ddpm {
 
-// Batched matmuls of the attention block (unet.py:43-51) and their adjoints.
-//   form 0 (NT): C[b][i][j] = alpha * sum_c A[b][i][c] * B[b][j][c]     M=i, N=j, K=c
-//   form 1 (NN): C[b][i][c] = sum_j A[b][i][j] * B[b][j][c]             M=i, N=c, K=j
-//   form 2 (TN): C[b][j][c] = sum_i A[b][i][j] * B[b][i][c]             M=j, N=c, K=i
-// A, B bf16 with row strides lda/ldb and per-batch strides = rows*ld; C bf16 or fp32.
-inline void UnetEngine::bmm(std::vector<Op>& L, const std::string& name, int form, const bf16* A, long long lda, long long sa,
-                            const bf16* Bp, long long ldb, long long sb, void* C, long long ldc, long long sc, bool c_f32,
-                            int nb, int T, int Cc, float alpha, double* fl_acc) {
-    // all attention products here are T x T x Cc shaped
-    const int M = T, N = (form == 0) ? T : Cc, K = (form == 0) ? Cc : T;
-    const double fl = 2.0 * nb * (double)M * N * K;
-    if (fl_acc) *fl_acc += fl;
-    const bool tc = (T % 128 == 0) && (Cc % 64 == 0) && ((T & (T - 1)) == 0);
-    if (tc) {
-        ddpm_gemm_desc d; memset(&d, 0, sizeof d);
-        d.M = M; d.N = N; d.W = T; d.H = 1; d.NB = nb; d.alpha = alpha; d.grid_z = nb;
-        d.out = C; d.ldo = (int)ldc; d.out_z_stride = sc; d.flags = c_f32 ? EPI_OUT_F32 : 0;
-        d.a_ptr[0] = A; d.a_ld[0] = lda;
-        if (form == 0) {
-            d.mode = GEMM_KK; d.a_C[0] = K; d.nseg = 1; d.seg_map[0] = 0; d.seg_taps[0] = 1; d.seg_kchunks[0] = K / 64; d.seg_cbase[0] = 0;
-            d.b_ptr = Bp; d.b_K = K; d.b_rows = N; d.b_batch = nb; d.b_ld = ldb; d.b_bs = sb; d.a_z_n = 1; d.b_z = 1;
-        } else if (form == 1) {
-            d.mode = GEMM_KMN; d.a_C[0] = K; d.b_ptr = Bp; d.b_K = N; d.b_ld = ldb; d.kblocks = K / 64; d.a_z_n = 1;
-        } else {
-            d.mode = GEMM_MNMN; d.a_C[0] = M; d.b_ptr = Bp; d.b_K = N; d.b_ld = ldb; d.taps = 1; d.splits = 1; d.kblocks = K / 64;
-        }
-        ++n_tc_gemms;
-        if (dry) { push(L, name, fl, [](cudaStream_t) { return 0; }); return; }
-        GemmLaunch g; int rc = build_gemm(d, g);
-        if (rc) { plan_error = rc; return; }
-        push(L, name, fl, [g](cudaStream_t st) { return launch_gemm(g, st); });
-        return;
+// the launch steps of an attention route (attn_fwd_steps / attn_bwd_steps) as ops named p + step.name
+inline void UnetEngine::push_attn_steps(std::vector<Op>& L, const std::string& p, const AttnSteps& steps, double& flops_acc) {
+    for (const AttnStep& s : steps) {
+        flops_acc += s.flops;
+        if (s.kind == ATTN_STEP_TC) ++n_tc_gemms;
+        else if (s.kind == ATTN_STEP_SIMT) ++n_generic;
+        push(L, p + s.name, s.flops, s.run);
     }
-    ++n_generic;
-    SgemmParams p; memset(&p, 0, sizeof p);
-    p.A = A; p.B = Bp; p.C = C; p.M = M; p.N = N; p.K = K; p.alpha = alpha;
-    p.sa_z = sa; p.sb_z = sb; p.sc_z = sc; p.sc_m = ldc; p.sc_n = 1;
-    if (form == 0) { p.sa_m = lda; p.sa_k = 1; p.sb_k = 1; p.sb_n = ldb; }
-    else if (form == 1) { p.sa_m = lda; p.sa_k = 1; p.sb_k = ldb; p.sb_n = 1; }
-    else { p.sa_m = 1; p.sa_k = lda; p.sb_k = ldb; p.sb_n = 1; }
-    const dim3 grid((N + 63) / 64, (M + 63) / 64, nb);
-    if (c_f32) push(L, name + "[simt]", fl, [p, grid](cudaStream_t st) { launch_k(k_sgemm<bf16, bf16, float>, grid, 256, 0, st, p); return (int)cudaGetLastError(); });
-    else       push(L, name + "[simt]", fl, [p, grid](cudaStream_t st) { launch_k(k_sgemm<bf16, bf16, bf16>, grid, 256, 0, st, p); return (int)cudaGetLastError(); });
 }
 
 // ResidualBlock (unet.py:63-89):  out = skip(x) + conv2(drop(silu(gn2(conv1(silu(gn1(x))) + fc(silu(temb))))))
@@ -125,7 +90,6 @@ inline T4 UnetEngine::res_block(const std::string& p, const Src& x, int cout, in
 // AttentionBlock (unet.py:23-60): out = x + Wo . softmax(Q^T K / sqrt(C)) V ,  q,k,v = chunk(Win . gn(x))
 inline T4 UnetEngine::attn_block(const std::string& p, const T4& x) {
     const int C = x.C, Bn = x.B, h = x.H, w = x.W, T = h * w;
-    const float scale = 1.f / sqrtf((float)C);
     T4 xn = newT(Bn, h, w, C);
     const GnSaved g = gn_fwd(fwd_ops, p + ".norm", one(x), p + ".norm", xn, 0, 0.f);
     const Packed win = pack_conv(p + ".project_in", 3 * C, C, 1, 0, false, true);
@@ -133,7 +97,6 @@ inline T4 UnetEngine::attn_block(const std::string& p, const T4& x) {
     { ConvSpec c; c.name = p + ".project_in"; c.in = one(xn); c.ksize = 1; c.wp = win.fwd; c.ldw = win.ld_f; c.bias = PP(p + ".project_in.bias");
       c.out = qkv; c.Co = 3 * C; c.Ho = h; c.Wo = w; conv_op(fwd_ops, c, &fwd_flops); }
     const bf16* q = bp(qkv);
-    const long long ldq = 3 * C, sq = (long long)T * 3 * C;
     T4 O = newT(Bn, h, w, C);
     float* S = nullptr; bf16* Pm = nullptr;
     static const bool no_fused_attn = getenv("DDPM_NO_FUSED_ATTN") != nullptr;
@@ -144,33 +107,17 @@ inline T4 UnetEngine::attn_block(const std::string& p, const T4& x) {
     const bool fused_attn_bwd = getenv("DDPM_FUSED_ATTN_BWD") != nullptr;
     const bool fused_bwd = train && fused_attn_bwd && !no_fused_attn && attn_fused_eligible(T, C);
     static const bool no_fused_attn_train = getenv("DDPM_NO_FUSED_ATTN_TRAIN") != nullptr;
-    if (!(train && no_fused_attn_train) && !no_fused_attn && attn_fused_eligible(T, C)) {
-        // Q.K^T -> softmax -> P.V in ONE kernel, S and O in registers, P in shared memory (attn_fused.cuh); training plans also get
-        // the normalised P in HBM for the backward pass
-        if (train) Pm = at<bf16>(alloc((size_t)Bn * T * T * 2));
-        const double fl = 4.0 * Bn * (double)T * T * C;
-        fwd_flops += fl; ++n_tc_gemms;
-        if (dry) push(fwd_ops, p + ".attn[fused]", fl, [](cudaStream_t) { return 0; });
-        else {
-            AttnLaunch g; const int rc = build_attn(q, bp(O), Bn, T, C, g, Pm);
-            if (rc) { plan_error = rc; return O; }
-            push(fwd_ops, p + ".attn[fused]", fl, [g](cudaStream_t st) { return launch_attn(g, st); });
-        }
-    } else if (small16) {
-        // 4x4 level: one CTA per image does scores, softmax and P.V (k_attn16_fwd); P is kept only when a backward follows
-        if (train) Pm = at<bf16>(alloc((size_t)Bn * T * T * 2));
-        const double fl = 4.0 * Bn * (double)T * T * C;
-        fwd_flops += fl; ++n_generic;
-        bf16* Op = bp(O); bf16* Pk = Pm; const size_t shm = attn16_smem(C, false);
-        if (!dry) cudaFuncSetAttribute(k_attn16_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn16_smem(512, false));
-        push(fwd_ops, p + ".attn[t16]", fl, [=](cudaStream_t st) { launch_k(k_attn16_fwd, Bn, 256, shm, st, q, Op, Pk, C, scale); return (int)cudaGetLastError(); });
-    } else {
-        S = at<float>(alloc((size_t)Bn * T * T * 4));
-        Pm = at<bf16>(alloc((size_t)Bn * T * T * 2));
-        bmm(fwd_ops, p + ".qk", 0, q, ldq, sq, q + C, ldq, sq, S, T, (long long)T * T, true, Bn, T, C, scale, &fwd_flops);
-        { const long long rows = (long long)Bn * T; const int nblk = (int)((rows + 7) / 8);
-          push(fwd_ops, p + ".softmax", 0, [=](cudaStream_t st) { launch_k(k_softmax_rows, nblk, 256, 0, st, S, Pm, rows, T); return (int)cudaGetLastError(); }); }
-        bmm(fwd_ops, p + ".pv", 1, Pm, T, (long long)T * T, q + 2 * C, ldq, sq, bp(O), C, (long long)T * C, false, Bn, T, C, 1.f, &fwd_flops);
+    const int route = (!(train && no_fused_attn_train) && !no_fused_attn && attn_fused_eligible(T, C)) ? ATTN_ROUTE_FUSED
+                    : small16 ? ATTN_ROUTE_T16 : ATTN_ROUTE_PRODUCTS;
+    // fused and t16 keep P (for the backward pass) only in training plans; the products route always materialises S and P
+    if (route == ATTN_ROUTE_PRODUCTS) S = at<float>(alloc((size_t)Bn * T * T * 4));
+    if (train || route == ATTN_ROUTE_PRODUCTS) Pm = at<bf16>(alloc((size_t)Bn * T * T * 2));
+    if (route == ATTN_ROUTE_T16 && !dry) { const int rc = attn16_prepare(); if (rc && !plan_error) plan_error = fail(-20, "attention '%s': %s", p.c_str(), cudaGetErrorString((cudaError_t)rc)); }
+    {
+        AttnSteps steps;
+        const int rc = attn_fwd_steps(steps, route, q, bp(O), Pm, S, Bn, T, C, dry);
+        if (rc) { plan_error = rc; return O; }
+        push_attn_steps(fwd_ops, p, steps, fwd_flops);
     }
     const Packed wout = pack_conv(p + ".project_out", C, C, 1, 0, false, true);
     T4 out = newT(Bn, h, w, C);
@@ -186,34 +133,15 @@ inline T4 UnetEngine::attn_block(const std::string& p, const T4& x) {
         wgrad_op(p + ".project_out.wgrad", dY, one(O), 1, 1, MAP_NORMAL, GP(p + ".project_out.weight"), C);
         T4 dqkv = newT(Bn, h, w, 3 * C);
         const bf16* dOp = bp(dO); bf16* dq = bp(dqkv);
-        if (small16) {
-            const double fl = 8.0 * Bn * (double)T * T * C;
-            bwd_flops += fl; ++n_generic;
-            const size_t shm = attn16_smem(C, true); const bf16* Pk = Pm;
-            if (!dry) cudaFuncSetAttribute(k_attn16_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn16_smem(512, true));
-            push(bwd_ops, p + ".attn_bwd[t16]", fl, [=](cudaStream_t st) { launch_k(k_attn16_bwd, Bn, 256, shm, st, q, dOp, Pk, dq, C, scale); return (int)cudaGetLastError(); });
-        } else if (fused_bwd) {
-            // dP -> softmax backward -> dQ in one launch (attn_kernel<true>); dK and dV read dS / P back as GEMM operands
-            bf16* dS = at<bf16>(alloc((size_t)Bn * T * T * 2));
-            const double fl = 4.0 * Bn * (double)T * T * C;
-            bwd_flops += fl; ++n_tc_gemms;
-            if (dry) push(bwd_ops, p + ".attn_bwd[fused]", fl, [](cudaStream_t) { return 0; });
-            else {
-                AttnLaunch g; const int rc = build_attn_bwd(q, dOp, Pm, dS, dq, Bn, T, C, g);
-                if (rc) { plan_error = rc; return; }
-                push(bwd_ops, p + ".attn_bwd[fused]", fl, [g](cudaStream_t st) { return launch_attn_bwd(g, st); });
-            }
-            bmm(bwd_ops, p + ".dV", 2, Pm, T, (long long)T * T, dOp, C, (long long)T * C, dq + 2 * C, ldq, sq, false, Bn, T, C, 1.f, &bwd_flops);
-            bmm(bwd_ops, p + ".dK", 2, dS, T, (long long)T * T, q, ldq, sq, dq + C, ldq, sq, false, Bn, T, C, 1.f, &bwd_flops);
-        } else {
-        float* dP = at<float>(alloc((size_t)Bn * T * T * 4));
-        bf16* dS = at<bf16>(alloc((size_t)Bn * T * T * 2));
-        bmm(bwd_ops, p + ".dP", 0, dOp, C, (long long)T * C, q + 2 * C, ldq, sq, dP, T, (long long)T * T, true, Bn, T, C, 1.f, &bwd_flops);
-        bmm(bwd_ops, p + ".dV", 2, Pm, T, (long long)T * T, dOp, C, (long long)T * C, dq + 2 * C, ldq, sq, false, Bn, T, C, 1.f, &bwd_flops);
-        { const long long rows = (long long)Bn * T; const int nblk = (int)((rows + 7) / 8);
-          push(bwd_ops, p + ".softmax_bwd", 0, [=](cudaStream_t st) { launch_k(k_softmax_bwd, nblk, 256, 0, st, Pm, dP, dS, rows, T, scale); return (int)cudaGetLastError(); }); }
-        bmm(bwd_ops, p + ".dQ", 1, dS, T, (long long)T * T, q + C, ldq, sq, dq, ldq, sq, false, Bn, T, C, 1.f, &bwd_flops);
-        bmm(bwd_ops, p + ".dK", 2, dS, T, (long long)T * T, q, ldq, sq, dq + C, ldq, sq, false, Bn, T, C, 1.f, &bwd_flops);
+        // t16 backward after a t16 forward; the fused dQ kernel only when opted in; the products route for every other shape
+        const int broute = small16 ? ATTN_ROUTE_T16 : fused_bwd ? ATTN_ROUTE_FUSED : ATTN_ROUTE_PRODUCTS;
+        float* dP = broute == ATTN_ROUTE_PRODUCTS ? at<float>(alloc((size_t)Bn * T * T * 4)) : nullptr;
+        bf16* dS = broute != ATTN_ROUTE_T16 ? at<bf16>(alloc((size_t)Bn * T * T * 2)) : nullptr;
+        {
+            AttnSteps steps;
+            const int rc = attn_bwd_steps(steps, broute, q, dOp, Pm, dP, dS, dq, Bn, T, C, dry);
+            if (rc) { plan_error = rc; return; }
+            push_attn_steps(bwd_ops, p, steps, bwd_flops);
         }
         colsum_op(p + ".project_in.bias", dqkv, nullptr, 0, GP(p + ".project_in.bias"), nullptr, 3 * C);
         T4 dxn = newT(Bn, h, w, C);

@@ -103,6 +103,34 @@ int ddpm_attn_fused_run(const void* qkv, void* out, void* probs, int NB, int T, 
  * d_qkv bf16 [NB][T][3C].  dK = dS^T Q and dV = P^T d_out are plain GEMMs over d_scores / probs (ddpm_gemm_run).  T = 256, C = 256. */
 int ddpm_attn_fused_bwd_run(const void* qkv, const void* d_out, const void* probs, void* d_scores, void* d_qkv, int NB, int T, int C, void* stream);
 
+/* Low-level operators: the attention core softmax(Q K^T / sqrt(C)) V of AttentionBlock (unet.py:43-51) and its backward, on any
+ * route the UNet engine's plans take, with the launch sequence those plans use (used by the parity tests of the engine itself).
+ * Routes (the engine picks one per attention block from the shape):
+ *  1  fused: attn_kernel<false>; backward attn_kernel<true> (dP, dS, dQ) + the dV and dK products.  T = 256, C = 256
+ *  2  t16: k_attn16_fwd / k_attn16_bwd, one CTA per image.  T = 16, C in {128, 256, 512}
+ *  3  products + row softmax: Q.K^T (fp32 S) -> k_softmax_rows -> P.V; backward dP (fp32), dV, k_softmax_bwd (dS), dQ, dK.  The
+ *     products run on the tensor cores when T is a power of two, T % 128 == 0 and C % 64 == 0, on CUDA cores otherwise.  Any T.
+ * qkv bf16 [NB][T][3C] (q | k | v, the chunk order of unet.py:57), out / d_out bf16 [NB][T][C], probs bf16 [NB][T][T] (forward:
+ * optional on routes 1 and 2, required and always written on route 3; backward: the probabilities a forward wrote, required),
+ * d_qkv bf16 [NB][T][3C] (all three thirds written), d_scores bf16 [NB][T][T] (optional; receives dS on routes 1 and 3, route 2
+ * does not form it in memory).  scratch: caller-owned device area of ddpm_attn_scratch_bytes(route, NB, T, C, backward) bytes (0
+ * when the route needs none: route 3's fp32 S / dP, and dS when d_scores is NULL).  C is a multiple of 8, 1 <= NB <= 65535,
+ * buffers are 16-byte aligned.  Arguments are checked before any device work. */
+typedef struct ddpm_attn_desc {
+    int route, NB, T, C;
+    const void* qkv; void* out; void* probs;
+    void* scratch;
+} ddpm_attn_desc;
+typedef struct ddpm_attn_bwd_desc {
+    int route, NB, T, C;
+    const void* qkv; const void* d_out; const void* probs;
+    void* d_qkv; void* d_scores;
+    void* scratch;
+} ddpm_attn_bwd_desc;
+int ddpm_attention_fwd_run(const ddpm_attn_desc* d, void* stream);
+int ddpm_attention_bwd_run(const ddpm_attn_bwd_desc* d, void* stream);
+long long ddpm_attn_scratch_bytes(int route, int NB, int T, int C, int backward);
+
 /* ------------------------------------------------------------------------------------------------
  * Low-level operators: GroupNorm(32, C, eps=1e-6) [+ SiLU] [+ dropout] (unet.py:18-20,83-84) and the bias column sums, with the
  * launch geometry the UNet engine's plans use (used by the parity tests of the engine itself).
