@@ -89,6 +89,26 @@ class AttnBwdDesc(C.Structure):
     ]
 
 
+class ConvReport(C.Structure):
+    _fields_ = [("route", C.c_int), ("launches", C.c_int), ("block_n", C.c_int), ("splits", C.c_int), ("zero_bytes", C.c_longlong)]
+
+
+class ConvDesc(C.Structure):
+    _fields_ = [
+        ("op", C.c_int), ("route", C.c_int),
+        ("B", C.c_int), ("H", C.c_int), ("W", C.c_int), ("ksize", C.c_int), ("stride", C.c_int), ("upsample", C.c_int),
+        ("Cin0", C.c_int), ("Cin1", C.c_int), ("Co", C.c_int), ("Cs0", C.c_int), ("Cs1", C.c_int), ("identity_skip", C.c_int),
+        ("x0", C.c_void_p), ("x1", C.c_void_p), ("s0", C.c_void_p), ("s1", C.c_void_p), ("dy", C.c_void_p),
+        ("w", C.c_void_p), ("w_skip", C.c_void_p),
+        ("bias", C.c_void_p), ("skip_bias", C.c_void_p), ("rowvec", C.c_void_p), ("rowvec_ld", C.c_int),
+        ("residual", C.c_void_p), ("accumulate", C.c_int),
+        ("out", C.c_void_p), ("qstats", C.c_void_p),
+        ("scratch", C.c_void_p),
+        ("dry", C.c_int),
+        ("report", C.POINTER(ConvReport)),
+    ]
+
+
 class UnetCfg(C.Structure):
     _fields_ = [("in_channels", C.c_int), ("hid_channels", C.c_int), ("out_channels", C.c_int),
                 ("levels", C.c_int), ("ch_mult", C.c_int * 8), ("num_res_blocks", C.c_int), ("attn", C.c_int * 8),
@@ -125,6 +145,8 @@ def lib():
             "ddpm_attention_fwd_run": ([C.POINTER(AttnDesc), vp], i32),
             "ddpm_attention_bwd_run": ([C.POINTER(AttnBwdDesc), vp], i32),
             "ddpm_attn_scratch_bytes": ([i32, i32, i32, i32, i32], i64),
+            "ddpm_conv_run": ([C.POINTER(ConvDesc), vp], i32),
+            "ddpm_conv_scratch_bytes": ([C.POINTER(ConvDesc)], i64),
             "ddpm_gn_scratch_bytes": ([i32, i32], i64),
             "ddpm_groupnorm_fwd_run": ([C.POINTER(GnDesc), vp], i32),
             "ddpm_groupnorm_bwd_run": ([C.POINTER(GnBwdDesc), vp], i32),
@@ -169,7 +191,7 @@ def lib():
 
 
 EXPORTS = ["ddpm_last_error", "ddpm_runtime_check", "ddpm_device_error_flag", "ddpm_gemm_run", "ddpm_conv_halo_run", "ddpm_attn_fused_run", "ddpm_attn_fused_bwd_run",
-           "ddpm_attention_fwd_run", "ddpm_attention_bwd_run", "ddpm_attn_scratch_bytes",
+           "ddpm_attention_fwd_run", "ddpm_attention_bwd_run", "ddpm_attn_scratch_bytes", "ddpm_conv_run", "ddpm_conv_scratch_bytes",
            "ddpm_gn_scratch_bytes", "ddpm_groupnorm_fwd_run", "ddpm_groupnorm_bwd_run", "ddpm_colsum_run",
            "ddpm_unet_create", "ddpm_unet_create_ex", "ddpm_unet_destroy", "ddpm_unet_num_params", "ddpm_unet_param_info",
            "ddpm_unet_flat_elems", "ddpm_unet_workspace_bytes", "ddpm_unet_plan", "ddpm_unet_repack",

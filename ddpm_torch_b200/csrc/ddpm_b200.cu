@@ -247,6 +247,187 @@ int ddpm_attention_bwd_run(const ddpm_attn_bwd_desc* d, void* stream) {
     return rc ? rc : attn_run(fn, steps, stream);
 }
 
+// ------------------------------------------------------------------------------------------------ convolutions
+// scratch layout: zero area (split-K fp32 [Ho*Wo*B][Co], or the 3x3 weight gradient's fp32 [9][Co][Cin]) | packed bf16 weights |
+// combined bias fp32 [Co] | pack table (PackEntry rows: the weight packs, then the gradient unpack)
+struct ConvPrep {
+    int op = 0, route = 0, Ho = 0, Wo = 0, Cin = 0;
+    ConvArgs a; ConvChoice ch; WgradArgs w;
+    long long ldp = 0;                  // row length of the packed weights
+    size_t zero_b = 0, pack_b = 0, bias_b = 0, table_b = 0;
+    size_t off_pack = 0, off_bias = 0, off_table = 0, total = 0;
+    int n_pack = 0; bool unpack = false, comb_bias = false;
+};
+static int conv_prepare(const char* fn, const ddpm_conv_desc* d, ConvPrep& p) {
+    if (!d) return fail(-44, "%s: null descriptor", fn);
+    if (d->op < 0 || d->op > 2) return fail(-44, "%s: op must be 0 (forward), 1 (data gradient) or 2 (weight gradient)", fn);
+    if (d->route < 1 || d->route > 5) return fail(-44, "%s: route must be 1 (halo), 2 (GEMM), 3 (CUDA cores), 4 (stride 2) or 5 (fold)", fn);
+    if (d->B < 1 || d->H < 1 || d->W < 1) return fail(-44, "%s: need B, H and W >= 1", fn);
+    if (d->B > 65535) return fail(-44, "%s: B = %d exceeds 65535", fn, d->B);
+    if (d->ksize != 1 && d->ksize != 3) return fail(-44, "%s: ksize must be 1 or 3", fn);
+    if (d->stride != 1 && d->stride != 2) return fail(-44, "%s: stride must be 1 or 2", fn);
+    if (d->upsample != 0 && d->upsample != 1) return fail(-44, "%s: upsample must be 0 or 1", fn);
+    if ((d->identity_skip != 0 && d->identity_skip != 1) || (d->accumulate != 0 && d->accumulate != 1) || (d->dry != 0 && d->dry != 1))
+        return fail(-44, "%s: identity_skip, accumulate and dry must be 0 or 1", fn);
+    if (d->Cin0 < 8 || d->Cin0 % 8 || d->Cin1 < 0 || d->Cin1 % 8 || d->Co < 8 || d->Co % 8 || d->Cs0 < 0 || d->Cs0 % 8 || d->Cs1 < 0 || d->Cs1 % 8)
+        return fail(-44, "%s: channel counts must be multiples of 8 (Cin0 and Co > 0)", fn);
+    if (d->Cs1 && !d->Cs0) return fail(-44, "%s: a second skip source needs a first (Cs0 > 0)", fn);
+    if (d->stride == 2 && (d->ksize != 3 || d->H % 2 || d->W % 2)) return fail(-44, "%s: stride 2 needs ksize 3 and an even H and W", fn);
+    if ((d->stride == 2 || d->upsample) && (d->Cin0 != d->Co || d->Cin1)) return fail(-44, "%s: the resample convs need one source with Cin0 = Co", fn);
+    if (d->upsample && (d->route != CONV_ROUTE_FOLD || d->op != 0 || d->ksize != 3 || d->stride != 1))
+        return fail(-44, "%s: upsample = 1 is the folded route 5 (forward of a 3x3 stride-1 conv)", fn);
+    if (d->route == CONV_ROUTE_FOLD && !d->upsample) return fail(-44, "%s: route 5 (fold) needs upsample = 1", fn);
+    const bool skip = d->Cs0 > 0 || d->identity_skip;
+    if (skip && (d->op != 0 || d->ksize != 3 || d->stride != 1 || d->upsample)) return fail(-44, "%s: a fused skip needs the forward of a 3x3 stride-1 conv", fn);
+    if (d->identity_skip && (d->Cs0 != d->Co || d->Cs1 || d->w_skip || d->skip_bias)) return fail(-44, "%s: identity_skip needs Cs0 = Co, Cs1 = 0, and no w_skip or skip_bias", fn);
+    if (d->skip_bias && (!d->Cs0 || d->identity_skip || !d->bias)) return fail(-44, "%s: skip_bias needs a 1x1 skip and a bias", fn);
+    if (d->op == 1 && d->Cin1) return fail(-44, "%s: the data gradient writes one dx tensor: Cin1 must be 0", fn);
+    if (d->op != 0 && (d->bias || d->rowvec || d->residual || d->qstats)) return fail(-44, "%s: gradients take no bias, rowvec, residual or qstats", fn);
+    if (d->op == 2 && d->accumulate) return fail(-44, "%s: the weight gradient takes no accumulate flag", fn);
+    if (d->rowvec && d->rowvec_ld < d->Co) return fail(-44, "%s: rowvec_ld must be >= Co", fn);
+    if (!d->out || (d->op != 1 && (!d->x0 || (d->Cin1 && !d->x1))) || (d->op != 0 && !d->dy) || (d->op != 2 && !d->w) ||
+        (d->Cs0 && !d->s0) || (d->Cs1 && !d->s1) || (d->Cs0 && !d->identity_skip && !d->w_skip))
+        return fail(-44, "%s: null buffer", fn);
+    for (const void* q : {d->x0, d->x1, d->s0, d->s1, d->dy, (const void*)d->w, (const void*)d->w_skip, (const void*)d->bias, (const void*)d->skip_bias,
+                          (const void*)d->rowvec, d->residual, (const void*)d->out, (const void*)d->qstats, (const void*)d->scratch})
+        if (misaligned16(q)) return fail(-44, "%s: buffers must be 16-byte aligned", fn);
+    p.op = d->op; p.route = d->route; p.Cin = d->Cin0 + d->Cin1;
+    p.Ho = d->upsample ? 2 * d->H : d->H / d->stride; p.Wo = d->upsample ? 2 * d->W : d->W / d->stride;
+    const int taps = d->ksize * d->ksize, B = d->B;
+    const bf16* x0 = static_cast<const bf16*>(d->x0); const bf16* x1 = static_cast<const bf16*>(d->x1);
+    const bf16* dy = static_cast<const bf16*>(d->dy);
+    int want = 0;                       // the planner's route for the shape
+    if (d->op == 2) {
+        WgradArgs& w = p.w;
+        w.dy = dy; w.B = B; w.Ho = p.Ho; w.Wo = p.Wo; w.Co = d->Co; w.Co_valid = d->Co;
+        w.in.x0 = x0; w.in.C0 = d->Cin0; w.in.x1 = d->Cin1 ? x1 : nullptr; w.in.C1 = d->Cin1; w.Hi = d->H; w.Wi = d->W;
+        w.ksize = d->ksize; w.stride = d->stride; w.map = MAP_NORMAL; w.dw = static_cast<float*>(d->out);
+        const bool tc = wgrad_route_tc(w);
+        want = !tc ? CONV_ROUTE_SIMT : (d->stride == 2 ? CONV_ROUTE_S2 : CONV_ROUTE_GEMM);
+        p.ch.route = want; p.ch.block_n = 64;
+        if (tc) p.ch.splits = wgrad_splits(w, d->Cin0, &p.ch.block_n);
+        if (tc && taps == 9) { p.zero_b = gn_align((size_t)9 * d->Co * p.Cin * 4); p.unpack = true; }
+    } else if (d->op == 0 && d->upsample) {
+        want = conv_fold_ok(d->Co, d->H, d->W) ? CONV_ROUTE_FOLD : 0;
+        if (!want) return fail(-44, "%s: route 5 (fold) needs Co %% 256 == 0 and an input map the tensor-core tiles cover (got %dx%d, Co = %d)", fn, d->H, d->W, d->Co);
+        p.ch.route = want; p.ch.block_n = pick_block_n(d->Co);
+        p.ldp = 16LL * d->Co; p.pack_b = gn_align((size_t)d->Co * p.ldp * 2); p.n_pack = 1;
+    } else if (d->op == 1 && d->stride == 2) {
+        const bool tc = conv_s2_dgrad_tc(d->Co, d->H, d->W);
+        want = tc ? CONV_ROUTE_S2 : CONV_ROUTE_SIMT;
+        p.ch.route = want; p.ch.block_n = tc ? pick_block_n(d->Co) : 64;
+        ConvArgs& a = p.a;                              // (CUDA cores: the transposed map over dY)
+        a.in.x0 = dy; a.in.C0 = d->Co; a.B = B; a.Hi = p.Ho; a.Wi = p.Wo; a.ksize = 3; a.map = MAP_TRANSPOSED2;
+        a.out = static_cast<bf16*>(d->out); a.Co = d->Cin0; a.Ho = d->H; a.Wo = d->W; a.accumulate = d->accumulate != 0;
+        p.ldp = 9LL * d->Co; p.pack_b = gn_align((size_t)d->Cin0 * p.ldp * 2); p.n_pack = 1;
+    } else {
+        ConvArgs& a = p.a;
+        a.B = B; a.ksize = d->ksize; a.stride = d->stride; a.map = MAP_NORMAL;
+        a.out = static_cast<bf16*>(d->out); a.accumulate = d->accumulate != 0;
+        if (d->op == 0) {
+            a.in.x0 = x0; a.in.C0 = d->Cin0; a.in.x1 = d->Cin1 ? x1 : nullptr; a.in.C1 = d->Cin1; a.Hi = d->H; a.Wi = d->W;
+            a.Co = d->Co; a.Ho = p.Ho; a.Wo = p.Wo;
+            a.has_skip = skip; a.skip_identity = d->identity_skip != 0;
+            a.skip.x0 = static_cast<const bf16*>(d->s0); a.skip.C0 = d->Cs0; a.skip.x1 = d->Cs1 ? static_cast<const bf16*>(d->s1) : nullptr; a.skip.C1 = d->Cs1;
+            a.rowvec = d->rowvec; a.rowvec_ld = d->rowvec_ld; a.residual = static_cast<const bf16*>(d->residual);
+            p.ldp = (long long)taps * p.Cin + d->Cs0 + d->Cs1; p.pack_b = gn_align((size_t)d->Co * p.ldp * 2);
+            p.n_pack = 1 + (skip ? 1 : 0);
+            if (d->skip_bias) { p.comb_bias = true; p.bias_b = gn_align((size_t)d->Co * 4); ++p.n_pack; }
+        } else {                                        // stride-1 data gradient: a conv over dY with the transposed (3x3: flipped) weights
+            a.in.x0 = dy; a.in.C0 = d->Co; a.Hi = d->H; a.Wi = d->W; a.Co = d->Cin0; a.Ho = d->H; a.Wo = d->W;
+            p.ldp = (long long)taps * d->Co; p.pack_b = gn_align((size_t)d->Cin0 * p.ldp * 2); p.n_pack = 1;
+        }
+        p.ch = conv_choose(a, d->route != CONV_ROUTE_GEMM, true);
+        want = p.ch.route;
+        if (p.ch.splits > 1) p.zero_b = gn_align((size_t)B * p.Ho * p.Wo * a.Co * 4);
+    }
+    if (d->route != want)
+        return fail(-44, "%s: route %d is not the route the planner takes for this shape (it takes route %d)", fn, d->route, want);
+    if (d->qstats) {
+        const bool route_ok = d->op == 0 && p.route != CONV_ROUTE_SIMT && p.ch.splits == 1;
+        const int hw = d->upsample ? d->H * d->W : p.Ho * p.Wo;
+        if (!route_ok || d->Co % 32 || hw % 32)
+            return fail(-44, "%s: qstats needs a forward on routes 1, 2 or 4 without split-K, or route 5, with Co %% 32 == 0 and a per-image pixel count %% 32 == 0", fn);
+    }
+    const int n_table = p.n_pack + (p.unpack ? 1 : 0);
+    p.table_b = gn_align((size_t)n_table * sizeof(PackEntry));
+    p.off_pack = p.zero_b; p.off_bias = p.off_pack + p.pack_b; p.off_table = p.off_bias + p.bias_b; p.total = p.off_table + p.table_b;
+    if (!d->dry && p.total && !d->scratch) return fail(-44, "%s: needs a scratch area of ddpm_conv_scratch_bytes bytes", fn);
+    return 0;
+}
+
+long long ddpm_conv_scratch_bytes(const ddpm_conv_desc* d) {
+    ConvPrep p;
+    if (!d) return fail(-44, "ddpm_conv_scratch_bytes: null descriptor");
+    ddpm_conv_desc q = *d; q.dry = 1;                  // sizes only: no scratch needed yet
+    const int rc = conv_prepare("ddpm_conv_scratch_bytes", &q, p);
+    return rc ? rc : (long long)p.total;
+}
+
+int ddpm_conv_run(const ddpm_conv_desc* d, void* stream) {
+    const char* fn = "ddpm_conv_run";
+    ConvPrep p;
+    int rc = conv_prepare(fn, d, p);
+    if (rc) return rc;
+    uint8_t* s = static_cast<uint8_t*>(d->scratch);
+    const bool dry = d->dry != 0;
+    float* zero = reinterpret_cast<float*>(s);
+    bf16* packed = reinterpret_cast<bf16*>(s + p.off_pack);
+    float* comb = reinterpret_cast<float*>(s + p.off_bias);
+    PackEntry* table = reinterpret_cast<PackEntry*>(s + p.off_table);
+    // the weight packs and the gradient unpack, as the plans' repack and unpack rows
+    std::vector<PackEntry> rows;
+    const int taps = d->ksize * d->ksize, Co = d->Co;
+    ConvSteps steps;
+    if (p.op == 0 && p.route == CONV_ROUTE_FOLD) {
+        rows.push_back(pack_upfold_entry(d->w, Co, packed, p.ldp));
+        rc = conv_fold_steps(steps, static_cast<const bf16*>(d->x0), d->B, d->H, d->W, Co, packed, p.ldp, d->bias,
+                             static_cast<bf16*>(d->out), d->qstats, dry);
+    } else if (p.op == 0) {
+        rows.push_back(pack_conv_entry(d->w, Co, p.Cin, taps, 0, packed, p.ldp, nullptr, 0, 0));
+        if (d->identity_skip) rows.push_back(pack_identity_entry(packed, p.ldp, taps * p.Cin, Co));
+        else if (d->Cs0) rows.push_back(pack_conv_entry(d->w_skip, Co, d->Cs0 + d->Cs1, 1, taps * p.Cin, packed, p.ldp, nullptr, 0, 0));
+        if (p.comb_bias) rows.push_back(pack_bias_add_entry(comb, d->bias, d->skip_bias, Co));
+        ConvArgs a = p.a; a.wp = packed; a.ldw = p.ldp; a.bias = p.comb_bias ? comb : d->bias; a.qstats = d->qstats;
+        rc = conv_fwd_steps(steps, a, p.ch, zero, dry);
+    } else if (p.op == 1) {
+        // dgrad pack [Cin][taps x Co]: 3x3 stride 1 flipped taps, 1x1 plain, stride 2 the parity blocks (tensor cores) or plain
+        const int dkind = d->stride == 2 ? (p.route == CONV_ROUTE_S2 ? 3 : 1) : (taps == 9 ? 2 : 1);
+        rows.push_back(pack_conv_entry(d->w, Co, d->Cin0, taps, 0, nullptr, 0, packed, p.ldp, dkind));
+        if (p.route == CONV_ROUTE_S2)
+            rc = conv_s2_dgrad_steps(steps, static_cast<const bf16*>(d->dy), d->B, d->H, d->W, Co, packed, p.ldp, static_cast<bf16*>(d->out),
+                                     d->accumulate != 0, dry);
+        else { ConvArgs a = p.a; a.wp = packed; a.ldw = p.ldp; rc = conv_fwd_steps(steps, a, p.ch, zero, dry); }
+    } else {
+        PackEntry un;
+        rc = wgrad_steps(steps, p.w, p.unpack ? zero : nullptr, &un, dry);
+        if (p.unpack) rows.push_back(un);
+    }
+    if (rc) return rc;
+    int launches = (p.n_pack ? 1 : 0) + (p.unpack ? 1 : 0);
+    for (const ConvStep& st : steps) launches += st.launches;
+    if (d->report) { d->report->route = p.route; d->report->launches = launches; d->report->block_n = p.ch.block_n; d->report->splits = p.ch.splits;
+                     d->report->zero_bytes = (long long)p.zero_b; }
+    if (dry) return 0;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    cudaError_t e = cudaSuccess;
+    if (!rows.empty() && (e = cudaMemcpyAsync(table, rows.data(), rows.size() * sizeof(PackEntry), cudaMemcpyHostToDevice, st)) != cudaSuccess)
+        return fail(-20, "%s: pack table upload failed: %s", fn, cudaGetErrorString(e));
+    if (p.n_pack) {
+        launch_k(k_pack_table, dim3(128, p.n_pack), 256, 0, st, (const PackEntry*)table);
+        if ((e = cudaGetLastError()) != cudaSuccess) return fail(-20, "%s: weight pack failed: %s", fn, cudaGetErrorString(e));
+    }
+    for (const ConvStep& c : steps) {
+        const int r = c.run(st);
+        if (r) return fail(-20, "%s: launch '%s' failed: %s", fn, c.name.c_str(), cudaGetErrorString((cudaError_t)r));
+    }
+    if (p.unpack) {
+        launch_k(k_pack_table, dim3(128, 1), 256, 0, st, (const PackEntry*)(table + p.n_pack));
+        if ((e = cudaGetLastError()) != cudaSuccess) return fail(-20, "%s: gradient unpack failed: %s", fn, cudaGetErrorString(e));
+    }
+    return 0;
+}
+
 // ------------------------------------------------------------------------------------------------ UNet engine
 int ddpm_unet_create(const ddpm_unet_cfg* cfg, ddpm_unet** out) { return ddpm_unet_create_ex(cfg, 1, out); }
 int ddpm_unet_create_ex(const ddpm_unet_cfg* cfg, int resample_with_conv, ddpm_unet** out) {

@@ -256,6 +256,313 @@ inline int attn_bwd_steps(AttnSteps& out, int route, const bf16* qkv, const bf16
     return attn_bmm(out, ".dK", 2, dS, T, tt, qkv, ldq, sq, dqkv + C, ldq, sq, false, NB, T, C, 1.f, dry);
 }
 
+// ------------------------------------------------------------------ convolution launches
+// The convolutions of the plans (conv_op, wgrad_op, the stride-2 data gradient of down_conv, the folded upsample of up_conv) and
+// the conv operator of the C ABI (ddpm_conv_run) are built by the functions below, so that both launch the same kernels with the
+// same descriptors, block_n and split counts over weights packed by the same PackEntry rows.  Routes:
+//   1 halo  3x3 stride 1 (+ fused 1x1 skip segments): conv_halo.cuh.  conv_route_tc + halo_eligible
+//   2 gemm  implicit GEMM on the tensor cores (GEMM_KK); split over K into a zeroed fp32 scratch + k_splitk_finalize when few output
+//           tiles; weight gradients GEMM_MNMN with fp32 atomics
+//   3 simt  k_conv_generic (+ a second launch for a skip), k_wgrad_generic: concat inputs, odd widths, MAP_TRANSPOSED2
+//   4 s2    stride-2 3x3 on the tensor cores: forward (a_estride 2), data gradient as four output-parity GEMMs (PK_CONV dkind 3),
+//           weight gradient (b_estride 2)
+//   5 fold  nearest-2x upsample folded into the 3x3 conv that follows it: four output-parity GEMMs over PK_UPFOLD weights
+enum { CONV_ROUTE_HALO = 1, CONV_ROUTE_GEMM = 2, CONV_ROUTE_SIMT = 3, CONV_ROUTE_S2 = 4, CONV_ROUTE_FOLD = 5 };
+// a launch step; kind counts as in AttnStep (tensor-core op, CUDA-core op, or neither: the skip launch of the CUDA-core route)
+struct ConvStep { std::string name; double flops; int kind; int launches; std::function<int(cudaStream_t)> run; };
+using ConvSteps = std::vector<ConvStep>;
+
+// Rows of the k_pack_table tables that lay out conv weights from the fp32 OIHW masters (the plans' repack and gradient unpack,
+// and the conv operator).
+//   PK_CONV      fwd [Co][ld_f] at column k_off (taps x Ci, tap-major) and / or dgr [Ci][ld_d] (dkind 1 plain, 2 flipped taps,
+//                3 stride-2 parity blocks); either may be null
+//   PK_IDENTITY  fwd[co][k_off + ci] = (co == ci)
+//   PK_BIAS_ADD  dst = a + b
+//   PK_UPFOLD    fwd [C][16C]: the nearest-2x upsample merged into the 3x3 weights, per output parity
+//   PK_UNPACK_GRAD  scratch [9][Co][Ci] -> dw OIHW, scratch cleared behind the read
+inline PackEntry pack_entry(int kind, int Co, int Ci, int taps) { PackEntry e; memset(&e, 0, sizeof e); e.kind = kind; e.Co = Co; e.Ci = Ci; e.taps = taps; return e; }
+inline PackEntry pack_conv_entry(const float* w, int Co, int Ci, int taps, int k_off, bf16* fwd, long long ld_f, bf16* dgr, long long ld_d, int dkind) {
+    PackEntry e = pack_entry(PK_CONV, Co, Ci, taps);
+    e.k_off = k_off; e.w = w; e.fwd = fwd; e.ld_f = ld_f; e.dgr = dgr; e.ld_d = ld_d; e.dkind = dgr ? dkind : 0;
+    return e;
+}
+inline PackEntry pack_identity_entry(bf16* fwd, long long ld_f, int k_off, int C) { PackEntry e = pack_entry(PK_IDENTITY, C, C, 1); e.k_off = k_off; e.fwd = fwd; e.ld_f = ld_f; return e; }
+inline PackEntry pack_bias_add_entry(float* dst, const float* a, const float* b, int n) { PackEntry e = pack_entry(PK_BIAS_ADD, n, 1, 1); e.w = a; e.w2 = b; e.fout = dst; return e; }
+inline PackEntry pack_upfold_entry(const float* w, int C, bf16* fwd, long long ld_f) { PackEntry e = pack_entry(PK_UPFOLD, C, C, 9); e.w = w; e.fwd = fwd; e.ld_f = ld_f; return e; }
+inline PackEntry unpack_grad_entry(float* scratch, float* dw, int Co, int Ci) { PackEntry e = pack_entry(PK_UNPACK_GRAD, Co, Ci, 9); e.fout = dw; e.scratch = scratch; return e; }
+
+// both box shapes the GEMM engine tiles NHWC maps with exist for an h x w map
+inline bool conv_tc_geom(int h, int w) { int a, b, c; return pick_box(w, h, 128, a, b, c) && pick_box(w, h, 64, a, b, c); }
+
+// out = conv(in) [+ 1x1 skip(skip)] + bias + rowvec[image] + residual, NHWC bf16 (accumulate: out += instead of a residual)
+struct ConvArgs {
+    GnSrc in{}; int B = 0, Hi = 0, Wi = 0;         // input concat (C1 = 0: one source) on an Hi x Wi map
+    int ksize = 3, stride = 1, map = MAP_NORMAL;
+    const bf16* wp = nullptr; long long ldw = 0;   // packed [Co][ldw]: taps x Cin, then the skip's K chunks
+    bool has_skip = false, skip_identity = false;  // skip_identity: the skip chunks carry identity weights (no FLOPs counted)
+    GnSrc skip{};
+    const float* bias = nullptr; const float* rowvec = nullptr; int rowvec_ld = 0; const bf16* residual = nullptr;
+    bf16* out = nullptr; int Co = 0, Ho = 0, Wo = 0; bool accumulate = false;
+    double* qstats = nullptr;                      // quad statistics of the output (halo and single-pass GEMM routes)
+    const float* xfK = nullptr; int xf_silu = 0;   // GroupNorm(+SiLU) folded into the operand path (halo route only)
+    int Cin() const { return in.C0 + in.C1; }
+    int skipC() const { return has_skip ? skip.C0 + skip.C1 : 0; }
+};
+struct ConvChoice { int route = 0; int block_n = 0; int splits = 1; bool n128 = false; };
+
+// SamePad2d(3,2) + 3x3 stride 2 (unet.py:163-167) on the tensor cores: tap offsets 0..2 on the stride-2 sampled input
+inline bool conv_s2_fwd(const ConvArgs& c) {
+    return c.stride == 2 && c.map == MAP_NORMAL && c.ksize == 3 && !c.has_skip && c.Ho * 2 == c.Hi && c.Wo * 2 == c.Wi;
+}
+// the tensor-core routes (halo, gemm, s2) take one NHWC source with 64-channel chunks on a map the GEMM engine can tile
+inline bool conv_route_tc(const ConvArgs& c) {
+    const bool s2 = conv_s2_fwd(c);
+    bool tc = (c.stride == 1 || s2) && c.map == MAP_NORMAL && c.in.C1 == 0 && c.in.C0 % 64 == 0 && c.Co % 64 == 0 &&
+              (s2 || (c.Ho == c.Hi && c.Wo == c.Wi)) && conv_tc_geom(c.Ho, c.Wo) && !(c.accumulate && c.residual);
+    if (c.has_skip) tc = tc && c.skip.C0 % 64 == 0 && c.skip.C1 % 64 == 0;
+    return tc;
+}
+// The planner's choice for a conv.  allow_halo = false is DDPM_NO_HALO; n128_fill = false is DDPM_NO_N128_FILL.
+inline ConvChoice conv_choose(const ConvArgs& c, bool allow_halo, bool n128_fill) {
+    ConvChoice r;
+    if (!conv_route_tc(c)) { r.route = CONV_ROUTE_SIMT; r.block_n = 64; return r; }
+    if (allow_halo && c.ksize == 3 && c.stride == 1 && halo_eligible(c.Ho, c.Wo, c.Co)) { r.route = CONV_ROUTE_HALO; r.block_n = pick_block_n(c.Co); return r; }
+    r.route = conv_s2_fwd(c) ? CONV_ROUTE_S2 : CONV_ROUTE_GEMM;
+    // small-M problems (8x8 / 4x4 levels) do not fill the SMs with output tiles: split the K loop across CTAs
+    // (fp32 atomics into a zeroed scratch) and finish bias / timestep vector / residual / bf16 in a tiny second kernel
+    const long long Pout = (long long)c.B * c.Ho * c.Wo;
+    int bn = pick_block_n(c.Co);
+    int tiles = (int)((Pout + 127) / 128) * ((c.Co + bn - 1) / bn);
+    // 8x8 levels: 64 tiles of 128x256 would need split-K (+ a finalize launch and fp32 atomics); 128 tiles of 128x128
+    // fill the machine in one wave with the same MMA time per CTA and no second pass
+    if (n128_fill && bn == 256 && tiles <= kPlanSms / 2 && tiles * 2 <= kPlanSms) { bn = 128; tiles *= 2; r.n128 = true; }
+    const int slabs = (int)(((long long)c.ksize * c.ksize * c.Cin() + c.skipC()) / 64);
+    int splits = 1;
+    // (a finalize launch + fp32 atomics cost more than a half-empty single wave: split only when under ~1/3 of the SMs have a tile)
+    if (tiles <= 48 && slabs >= 16) { splits = kPlanSms / tiles; if (splits > slabs / 8) splits = slabs / 8; if (splits > 16) splits = 16; if (splits < 1) splits = 1; }
+    r.block_n = bn; r.splits = splits;
+    return r;
+}
+inline double conv_flops(const ConvArgs& c) {
+    const long long Pout = (long long)c.B * c.Ho * c.Wo;
+    return 2.0 * Pout * c.Co * (double)(c.ksize * c.ksize * c.Cin() + (c.skip_identity ? 0 : c.skipC()));
+}
+// the launch steps of route ch.route; splitk_scratch: zeroed fp32 [B*Ho*Wo][Co] when ch.splits > 1 (left zeroed)
+inline int conv_fwd_steps(ConvSteps& S, const ConvArgs& c, const ConvChoice& ch, float* splitk_scratch, bool dry) {
+    const int Cin = c.Cin(), taps = c.ksize * c.ksize;
+    const long long Pout = (long long)c.B * c.Ho * c.Wo;
+    const double fl = conv_flops(c);
+    const long long K = (long long)taps * Cin + c.skipC();
+    const bf16* resid = c.accumulate ? c.out : c.residual;
+    if (ch.route == CONV_ROUTE_HALO) {
+        ddpm_halo_desc h; memset(&h, 0, sizeof h);
+        h.NB = c.B; h.H = c.Ho; h.W = c.Wo; h.Cout = c.Co;
+        h.a_ptr[0] = c.in.x0; h.a_C[0] = c.in.C0; h.a_ld[0] = c.in.C0;
+        h.nseg = 1; h.seg_map[0] = 0; h.seg_taps[0] = 9; h.seg_kchunks[0] = c.in.C0 / 64; h.seg_cbase[0] = 0;
+        if (c.has_skip) {
+            h.a_ptr[1] = c.skip.x0; h.a_C[1] = c.skip.C0; h.a_ld[1] = c.skip.C0;
+            h.seg_map[1] = 1; h.seg_taps[1] = 1; h.seg_kchunks[1] = c.skip.C0 / 64; h.seg_cbase[1] = 0; h.nseg = 2;
+            if (c.skip.C1) {
+                h.a_ptr[2] = c.skip.x1; h.a_C[2] = c.skip.C1; h.a_ld[2] = c.skip.C1;
+                h.seg_map[2] = 2; h.seg_taps[2] = 1; h.seg_kchunks[2] = c.skip.C1 / 64; h.seg_cbase[2] = 0; h.nseg = 3;
+            }
+        }
+        h.w = c.wp; h.ldw = c.ldw; h.Ktot = (int)K; h.out = c.out; h.bias = c.bias; h.rowvec = c.rowvec; h.rowvec_ld = c.rowvec_ld;
+        h.residual = resid; h.base_offset_mode = 0; h.gn.qstats = c.qstats;
+        if (c.xfK) { h.xf_K = c.xfK; h.xf_silu = c.xf_silu; h.force_sub = 3; }
+        if (dry) { S.push_back({"[halo]", fl, ATTN_STEP_TC, 1, [](cudaStream_t) { return 0; }}); return 0; }
+        HaloLaunch g; const int rc = build_halo(h, g);
+        if (rc) return rc;
+        S.push_back({"[halo]", fl, ATTN_STEP_TC, 1, [g](cudaStream_t st) { return launch_halo(g, st); }});
+        return 0;
+    }
+    if (ch.route == CONV_ROUTE_GEMM || ch.route == CONV_ROUTE_S2) {
+        ddpm_gemm_desc d; memset(&d, 0, sizeof d);
+        d.mode = GEMM_KK; d.M = (int)Pout; d.N = c.Co; d.W = c.Wo; d.H = c.Ho; d.NB = c.B;
+        d.a_ptr[0] = c.in.x0; d.a_C[0] = c.in.C0; d.a_ld[0] = c.in.C0;
+        d.nseg = 1; d.seg_map[0] = 0; d.seg_taps[0] = taps; d.seg_kchunks[0] = c.in.C0 / 64; d.seg_cbase[0] = 0;
+        if (ch.route == CONV_ROUTE_S2) {   // SamePad2d(3,2): pad bottom/right only -> tap offsets 0..2 on the stride-2 sampled map, OOB = zero fill
+            d.a_estride = 2; d.seg_custom[0] = 1; d.seg_cmul[0] = 2;
+            for (int t = 0; t < 9; ++t) { d.seg_dx[0][t] = (signed char)(t % 3); d.seg_dy[0][t] = (signed char)(t / 3); }
+        }
+        if (c.has_skip) {
+            d.a_ptr[1] = c.skip.x0; d.a_C[1] = c.skip.C0; d.a_ld[1] = c.skip.C0;
+            d.seg_map[1] = 1; d.seg_taps[1] = 1; d.seg_kchunks[1] = c.skip.C0 / 64; d.seg_cbase[1] = 0; d.nseg = 2;
+            if (c.skip.C1) {
+                d.a_ptr[2] = c.skip.x1; d.a_C[2] = c.skip.C1; d.a_ld[2] = c.skip.C1;
+                d.seg_map[2] = 2; d.seg_taps[2] = 1; d.seg_kchunks[2] = c.skip.C1 / 64; d.seg_cbase[2] = 0; d.nseg = 3;
+            }
+        }
+        d.b_ptr = c.wp; d.b_K = (int)K; d.b_rows = c.Co; d.b_batch = 1; d.b_ld = c.ldw; d.b_bs = 0;
+        d.out = c.out; d.ldo = c.Co; d.alpha = 1.f; d.grid_z = 1;
+        d.bias = c.bias; d.rowvec = c.rowvec; d.rowvec_ld = c.rowvec_ld; d.rows_per_vec = c.Ho * c.Wo;
+        d.residual = resid; d.ldr = c.Co;
+        if (ch.n128) d.block_n = 128;
+        if (ch.splits > 1) {
+            if (!splitk_scratch && !dry) return fail(-31, "internal: split-K conv without its scratch");
+            ddpm_gemm_desc ds = d;
+            ds.kk_splits = ch.splits; ds.grid_z = ch.splits; ds.out = splitk_scratch; ds.flags = EPI_OUT_F32 | EPI_ATOMIC;
+            ds.bias = nullptr; ds.rowvec = nullptr; ds.residual = nullptr;
+            if (dry) { S.push_back({"[splitk]", fl, ATTN_STEP_TC, 2, [](cudaStream_t) { return 0; }}); return 0; }
+            const float* bias = c.bias; const float* rowvec = c.rowvec; const int rvld = c.rowvec_ld, rpv = c.Ho * c.Wo;
+            float* scratch = splitk_scratch; bf16* outp = c.out;
+            const long long M = Pout; const int N = c.Co; const int nfin = grid_for(M * (N / 8));
+            GemmLaunch g; const int rc = build_gemm(ds, g);
+            if (rc) return rc;
+            S.push_back({"[splitk]", fl, ATTN_STEP_TC, 2, [=](cudaStream_t st) {
+                const int r2 = launch_gemm(g, st); if (r2) return r2;
+                launch_k(k_splitk_finalize, nfin, 256, 0, st, scratch, bias, rowvec, rvld, rpv, resid, outp, M, N);
+                return (int)cudaGetLastError(); }});
+            return 0;
+        }
+        d.gn.qstats = c.qstats;
+        if (dry) { S.push_back({"", fl, ATTN_STEP_TC, 1, [](cudaStream_t) { return 0; }}); return 0; }
+        GemmLaunch g; const int rc = build_gemm(d, g);
+        if (rc) return rc;
+        S.push_back({"", fl, ATTN_STEP_TC, 1, [g](cudaStream_t st) { return launch_gemm(g, st); }});
+        return 0;
+    }
+    ConvG g; memset(&g, 0, sizeof g);
+    g.in = c.in; g.wp = c.wp; g.ldw = c.ldw; g.bias = c.bias; g.rowvec = c.rowvec; g.rowvec_ld = c.rowvec_ld;
+    g.residual = c.residual; g.out = c.out; g.out_nchw_f32 = 0;
+    g.B = c.B; g.Hi = c.Hi; g.Wi = c.Wi; g.Ho = c.Ho; g.Wo = c.Wo; g.Co = c.Co; g.ksize = c.ksize; g.stride = c.stride;
+    g.pad = (c.map == MAP_NORMAL && c.stride == 1) ? c.ksize / 2 : 0; g.map = c.map; g.accumulate = c.accumulate ? 1 : 0;
+    const dim3 grid((unsigned)((Pout + 63) / 64), (unsigned)((c.Co + 63) / 64));
+    S.push_back({"[simt]", fl, ATTN_STEP_SIMT, 1, [g, grid](cudaStream_t st) { launch_k(k_conv_generic, grid, 256, 0, st, g); return (int)cudaGetLastError(); }});
+    if (c.has_skip) {
+        ConvG s = g; s.in = c.skip; s.wp = c.wp + (long long)taps * Cin; s.ksize = 1; s.pad = 0; s.map = MAP_NORMAL; s.stride = 1;
+        s.bias = nullptr; s.rowvec = nullptr; s.residual = nullptr; s.accumulate = 1;
+        S.push_back({".skip[simt]", 0, ATTN_STEP_AUX, 1, [s, grid](cudaStream_t st) { launch_k(k_conv_generic, grid, 256, 0, st, s); return (int)cudaGetLastError(); }});
+    }
+    return 0;
+}
+
+// Data gradient of the stride-2 conv (down_conv) on the tensor cores: four output-parity sub-convolutions over dY (4 + 2 + 2 + 1
+// taps) whose epilogues scatter to the (2y+py, 2x+px) pixels of dx [B][h][w][C], reading the PK_CONV dkind-3 pack [C][9C]
+// (accumulate: dx += as a residual read of dx itself)
+inline bool conv_s2_dgrad_tc(int C, int h, int w) { return (C % 64 == 0) && conv_tc_geom(h / 2, w / 2); }
+inline int conv_s2_dgrad_steps(ConvSteps& S, const bf16* dY, int B, int h, int w, int C, const bf16* wd, long long ld_d, bf16* dx, bool accumulate, bool dry) {
+    const double fl = 2.0 * ((long long)B * (h / 2) * (w / 2)) * C * 9.0 * C;
+    int q = 0;
+    for (int py = 0; py < 2; ++py) for (int px = 0; px < 2; ++px, ++q) {
+        ddpm_gemm_desc d; memset(&d, 0, sizeof d);
+        d.mode = GEMM_KK; d.M = B * (h / 2) * (w / 2); d.N = C; d.W = w / 2; d.H = h / 2; d.NB = B;
+        d.a_ptr[0] = dY; d.a_C[0] = C; d.a_ld[0] = C;
+        d.nseg = 1; d.seg_map[0] = 0; d.seg_kchunks[0] = C / 64; d.seg_cbase[0] = 0; d.seg_custom[0] = 1; d.seg_cmul[0] = 1;
+        int nt = 0;
+        for (int ky = py ? 1 : 0; ky < 3; ky += 2) for (int kx = px ? 1 : 0; kx < 3; kx += 2) {
+            d.seg_dy[0][nt] = (signed char)(-(ky / 2)); d.seg_dx[0][nt] = (signed char)(-(kx / 2)); ++nt;
+            if (px) break;
+        }
+        // (the loops above enumerate ky in {0,2} or {1} and kx in {0,2} or {1}, kx fastest)
+        d.seg_taps[0] = nt;
+        d.b_ptr = wd; d.b_K = 9 * C; d.b_rows = C; d.b_batch = 1; d.b_ld = ld_d;
+        d.b_k_base = (py == 0 ? (px == 0 ? 0 : 4) : (px == 0 ? 6 : 8)) * C;
+        d.out = dx; d.ldo = C; d.alpha = 1.f; d.grid_z = 1; d.o_mul = 2; d.o_py = py; d.o_px = px;
+        if (accumulate) { d.residual = dx; d.ldr = C; }
+        if (dry) { S.push_back({"", q ? 0 : fl, ATTN_STEP_TC, 1, [](cudaStream_t) { return 0; }}); continue; }
+        GemmLaunch g; const int rc = build_gemm(d, g);
+        if (rc) return rc;
+        S.push_back({"", q ? 0 : fl, ATTN_STEP_TC, 1, [g](cudaStream_t st) { return launch_gemm(g, st); }});
+    }
+    return 0;
+}
+
+// Nearest-2x upsample + 3x3 conv (unet.py:199-202) with the upsampled tensor never materialised: four output-parity
+// sub-convolutions with 2x2 taps over the low-resolution x [B][h][w][C] (merged weights, PK_UPFOLD [C][16C]) scatter to the
+// (2y+py, 2x+px) pixels of out [B][2h][2w][C]: 4/9 of the MACs, no 2x copy.  qstats: the output's quad statistics (or null).
+inline bool conv_fold_ok(int C, int h, int w) { return C % 256 == 0 && conv_tc_geom(h, w); }
+inline int conv_fold_steps(ConvSteps& S, const bf16* x, int B, int h, int w, int C, const bf16* wf, long long ld_f, const float* bias,
+                           bf16* out, double* qstats, bool dry) {
+    const double fl = 2.0 * ((long long)B * 4 * h * w) * C * 9.0 * C;       // the reference's count (the folded form does 4/9 of it)
+    for (int q = 0; q < 4; ++q) {
+        const int py = q >> 1, px = q & 1;
+        ddpm_gemm_desc d; memset(&d, 0, sizeof d);
+        d.mode = GEMM_KK; d.M = B * h * w; d.N = C; d.W = w; d.H = h; d.NB = B;
+        d.a_ptr[0] = x; d.a_C[0] = C; d.a_ld[0] = C;
+        d.nseg = 1; d.seg_map[0] = 0; d.seg_kchunks[0] = C / 64; d.seg_cbase[0] = 0; d.seg_custom[0] = 1; d.seg_cmul[0] = 1; d.seg_taps[0] = 4;
+        for (int a = 0; a < 2; ++a) for (int b = 0; b < 2; ++b) {
+            d.seg_dy[0][a * 2 + b] = (signed char)(py == 0 ? a - 1 : a); d.seg_dx[0][a * 2 + b] = (signed char)(px == 0 ? b - 1 : b);
+        }
+        d.b_ptr = wf; d.b_K = 16 * C; d.b_rows = C; d.b_batch = 1; d.b_ld = ld_f; d.b_k_base = q * 4 * C;
+        d.out = out; d.ldo = C; d.alpha = 1.f; d.grid_z = 1; d.o_mul = 2; d.o_py = py; d.o_px = px;
+        d.bias = bias; d.gn.qstats = qstats;
+        if (dry) { S.push_back({"[fold]", q ? 0 : fl, ATTN_STEP_TC, 1, [](cudaStream_t) { return 0; }}); continue; }
+        GemmLaunch g; const int rc = build_gemm(d, g);
+        if (rc) return rc;
+        S.push_back({"[fold]", q ? 0 : fl, ATTN_STEP_TC, 1, [g](cudaStream_t st) { return launch_gemm(g, st); }});
+    }
+    return 0;
+}
+
+// weight gradient dW (OIHW fp32) of a conv from dy [B][Ho][Wo][Co] and the conv input `in` on an Hi x Wi map
+struct WgradArgs {
+    const bf16* dy = nullptr; int B = 0, Ho = 0, Wo = 0, Co = 0, Co_valid = 0;
+    GnSrc in{}; int Hi = 0, Wi = 0;
+    int ksize = 3, stride = 1, map = MAP_NORMAL;
+    float* dw = nullptr;
+    int Cin() const { return in.C0 + in.C1; }
+};
+inline bool wgrad_s2(const WgradArgs& w) { return w.stride == 2 && w.ksize == 3 && w.in.C1 == 0 && w.Hi == 2 * w.Ho && w.Wi == 2 * w.Wo; }
+inline bool wgrad_route_tc(const WgradArgs& w) {
+    const bool s2 = wgrad_s2(w);
+    return (w.stride == 1 || s2) && w.map == MAP_NORMAL && w.Co % 64 == 0 && w.Co == w.Co_valid && w.in.C0 % 64 == 0 && w.in.C1 % 64 == 0 &&
+           conv_tc_geom(w.Ho, w.Wo) && (s2 || w.Hi == w.Ho);
+}
+// split count of source s of a tensor-core weight gradient: ONE full wave (<= kPlanSms CTAs), since more splits only add epilogue
+// atomics and kPlanSms*k + 1 CTAs would cost a whole extra wave (1x1 weight gradients are a few output tiles and HBM-bound: half a
+// wave leaves the other SMs to the main chain)
+inline int wgrad_splits(const WgradArgs& w, int Cs, int* block_n) {
+    const int taps = w.ksize * w.ksize, kblocks = (int)(((long long)w.B * w.Ho * w.Wo + 63) / 64);
+    const int bn = pick_block_n(Cs);
+    const int tiles = ((w.Co + 127) / 128) * (Cs / bn) * taps;
+    int splits = ((taps == 1 && tiles <= 12) ? kPlanSms / 2 : kPlanSms) / tiles; if (splits > kblocks / 4) splits = kblocks / 4; if (splits < 1) splits = 1;
+    if (block_n) *block_n = bn;
+    return splits;
+}
+// Tensor-core route: one MNMN GEMM per concat source (fp32 atomics: 1x1 into dw, which must hold zeros or the sum so far; 3x3 into
+// scratch9 = zeroed [9][Co][Cin], after which *unpack, a PK_UNPACK_GRAD row, writes dw and clears the scratch).
+// CUDA cores: k_wgrad_generic, accumulating into dw.
+inline int wgrad_steps(ConvSteps& S, const WgradArgs& w, float* scratch9, PackEntry* unpack, bool dry) {
+    const int Cin = w.Cin(), taps = w.ksize * w.ksize, Co = w.Co;
+    const long long P = (long long)w.B * w.Ho * w.Wo;
+    const double fl = 2.0 * P * w.Co_valid * (double)taps * Cin;
+    if (wgrad_route_tc(w)) {
+        const bool s2 = wgrad_s2(w);
+        if (taps == 9 && !scratch9 && !dry) return fail(-31, "internal: 3x3 weight gradient without its scratch");
+        for (int s = 0; s < (w.in.C1 ? 2 : 1); ++s) {
+            const bf16* a = s ? w.in.x1 : w.in.x0; const int Cs = s ? w.in.C1 : w.in.C0, coff = s ? w.in.C0 : 0;
+            ddpm_gemm_desc d; memset(&d, 0, sizeof d);
+            d.mode = GEMM_MNMN; d.M = Co; d.N = Cs; d.W = w.Wo; d.H = w.Ho; d.NB = w.B;
+            d.a_ptr[0] = w.dy; d.a_C[0] = Co; d.a_ld[0] = Co;
+            d.b_ptr = a; d.b_K = Cs; d.b_ld = Cs;
+            if (s2) { d.b_estride = 2; d.b_pad = 0; }
+            d.taps = taps; d.kblocks = (int)((P + 63) / 64);
+            d.splits = wgrad_splits(w, Cs, nullptr); d.grid_z = taps * d.splits;
+            d.flags = EPI_OUT_F32 | EPI_ATOMIC; d.alpha = 1.f;
+            if (taps == 9) { d.out = scratch9 + coff; d.ldo = Cin; d.out_tap_stride = (long long)Co * Cin; }
+            else { d.out = w.dw + coff; d.ldo = Cin; }
+            if (dry) { S.push_back({"", s ? 0 : fl, ATTN_STEP_TC, 1, [](cudaStream_t) { return 0; }}); continue; }
+            GemmLaunch g; const int rc = build_gemm(d, g);
+            if (rc) return rc;
+            S.push_back({"", s ? 0 : fl, ATTN_STEP_TC, 1, [g](cudaStream_t st) { return launch_gemm(g, st); }});
+        }
+        if (taps == 9 && unpack) *unpack = unpack_grad_entry(scratch9, w.dw, Co, Cin);
+        return 0;
+    }
+    WgradG g; memset(&g, 0, sizeof g);
+    g.dy = w.dy; g.in = w.in; g.dw = w.dw; g.s_co = (long long)Cin * taps; g.s_ci = taps; g.s_tap = 1;
+    g.B = w.B; g.Hi = w.Hi; g.Wi = w.Wi; g.Ho = w.Ho; g.Wo = w.Wo; g.Co = Co; g.ksize = w.ksize; g.stride = w.stride;
+    g.pad = (w.map == MAP_NORMAL && w.stride == 1) ? w.ksize / 2 : 0; g.map = w.map; g.Co_valid = w.Co_valid;
+    const int tiles = ((Cin + 63) / 64) * ((Co + 63) / 64) * taps;
+    int splits = (592 + tiles - 1) / tiles; const int maxs = (int)((P + 255) / 256); if (splits > maxs) splits = maxs; if (splits < 1) splits = 1;
+    g.pix_per_split = (int)(((P + splits - 1) / splits + 15) / 16 * 16);
+    splits = (int)((P + g.pix_per_split - 1) / g.pix_per_split);
+    const dim3 grid((Cin + 63) / 64, (Co + 63) / 64, taps * splits);
+    S.push_back({"[simt]", fl, ATTN_STEP_SIMT, 1, [g, grid](cudaStream_t st) { launch_k(k_wgrad_generic, grid, 256, 0, st, g); return (int)cudaGetLastError(); }});
+    return 0;
+}
+
 struct UnetEngine {
     ddpm_unet_cfg cfg;
     bool resample_with_conv = true;       // false: AvgPool2d(2) / bare nearest x2 instead of the resample convs (unet.py:164-170,199-202)
@@ -397,7 +704,7 @@ struct UnetEngine {
     bool has_grad(const T4& t) const { auto it = grads.find(t.off); return it != grads.end() && it->second.second; }
 
     // ------------------------------------------------------------------ op builders
-    bool tc_ok_geom(int h, int w) const { int a, b, c; return pick_box(w, h, 128, a, b, c) && pick_box(w, h, 64, a, b, c); }
+    bool tc_ok_geom(int h, int w) const { return conv_tc_geom(h, w); }
 
     // conv: out = conv(in) [+ 1x1 skip(skip_in)] + bias + rowvec[b] + residual ; packed weights [Co][ldw]
     struct ConvSpec {
@@ -405,7 +712,7 @@ struct UnetEngine {
         const bf16* wp = nullptr; long long ldw = 0; bool has_skip = false; Src skip_in;
         bool skip_identity = false;        // the skip chunks carry identity weights (the block's residual): no FLOPs of the reference's count
         const float* bias = nullptr; const float* rowvec = nullptr; int rowvec_ld = 0; const bf16* residual = nullptr;
-        T4 out; float* out_nchw = nullptr; int Co = 0; int Ho = 0, Wo = 0; bool accumulate = false;
+        T4 out; int Co = 0; int Ho = 0, Wo = 0; bool accumulate = false;
         bool want_qstats = false;          // the output feeds a GroupNorm -> statistics in the epilogue when the kernel can
         const float* xfK = nullptr; int xf_silu = 0;   // inference: `in` is the RAW GroupNorm input, the conv applies act(sc*x + sh) in its
                                                        // operand path (haloed kernel only; see xf_ok / gn_prep_xf)
@@ -443,123 +750,34 @@ struct UnetEngine {
         }
         return qs;
     }
+    // the launch steps of a conv builder as ops named name + step.name; side: forked onto the side stream
+    void push_conv_steps(std::vector<Op>& L, const std::string& name, const ConvSteps& steps, double* flops_acc, bool side = false) {
+        for (const ConvStep& s : steps) {
+            if (flops_acc) *flops_acc += s.flops;
+            if (s.kind == ATTN_STEP_TC) ++n_tc_gemms;
+            else if (s.kind == ATTN_STEP_SIMT) ++n_generic;
+            push(L, name + s.name, s.flops, s.run, s.launches, side);
+        }
+    }
     long long conv_op(std::vector<Op>& L, const ConvSpec& c, double* flops_acc) {
-        const int Cin = c.in.C(), taps = c.ksize * c.ksize;
-        const T4& i0 = c.in.t0;
-        const int Bn = i0.B;
-        const long long Pout = (long long)Bn * c.Ho * c.Wo;
-        double fl = 2.0 * Pout * c.Co * (double)(taps * Cin + ((c.has_skip && !c.skip_identity) ? c.skip_in.C() : 0));
-        if (flops_acc) *flops_acc += fl;
-        const bool s2 = c.stride == 2 && c.map == MAP_NORMAL && c.ksize == 3 && !c.has_skip && c.Ho * 2 == i0.H && c.Wo * 2 == i0.W;
-        bool tc = (c.stride == 1 || s2) && c.map == MAP_NORMAL && !c.out_nchw && !c.in.two && (i0.C % 64 == 0) && (c.Co % 64 == 0) &&
-                  (s2 || (c.Ho == i0.H && c.Wo == i0.W)) && tc_ok_geom(c.Ho, c.Wo) && !(c.accumulate && c.residual);
-        if (c.has_skip) tc = tc && (c.skip_in.t0.C % 64 == 0) && (!c.skip_in.two || c.skip_in.t1.C % 64 == 0);
+        ConvArgs a;
+        a.in = gsrc(c.in); a.B = c.in.t0.B; a.Hi = c.in.t0.H; a.Wi = c.in.t0.W; a.ksize = c.ksize; a.stride = c.stride; a.map = c.map;
+        a.wp = c.wp; a.ldw = c.ldw; a.has_skip = c.has_skip; a.skip_identity = c.skip_identity;
+        if (c.has_skip) a.skip = gsrc(c.skip_in);
+        a.bias = c.bias; a.rowvec = c.rowvec; a.rowvec_ld = c.rowvec_ld; a.residual = c.residual;
+        a.out = bp(c.out); a.Co = c.Co; a.Ho = c.Ho; a.Wo = c.Wo; a.accumulate = c.accumulate; a.xfK = c.xfK; a.xf_silu = c.xf_silu;
         static const bool no_halo = getenv("DDPM_NO_HALO") != nullptr;
-        if (tc && !no_halo && c.ksize == 3 && c.stride == 1 && halo_eligible(c.Ho, c.Wo, c.Co)) {
-            ddpm_halo_desc h; memset(&h, 0, sizeof h);
-            h.NB = Bn; h.H = c.Ho; h.W = c.Wo; h.Cout = c.Co;
-            h.a_ptr[0] = bp(i0); h.a_C[0] = i0.C; h.a_ld[0] = i0.C;
-            h.nseg = 1; h.seg_map[0] = 0; h.seg_taps[0] = 9; h.seg_kchunks[0] = i0.C / 64; h.seg_cbase[0] = 0;
-            long long K = 9LL * Cin;
-            if (c.has_skip) {
-                h.a_ptr[1] = bp(c.skip_in.t0); h.a_C[1] = c.skip_in.t0.C; h.a_ld[1] = c.skip_in.t0.C;
-                h.seg_map[1] = 1; h.seg_taps[1] = 1; h.seg_kchunks[1] = c.skip_in.t0.C / 64; h.seg_cbase[1] = 0; h.nseg = 2; K += c.skip_in.t0.C;
-                if (c.skip_in.two) {
-                    h.a_ptr[2] = bp(c.skip_in.t1); h.a_C[2] = c.skip_in.t1.C; h.a_ld[2] = c.skip_in.t1.C;
-                    h.seg_map[2] = 2; h.seg_taps[2] = 1; h.seg_kchunks[2] = c.skip_in.t1.C / 64; h.seg_cbase[2] = 0; h.nseg = 3; K += c.skip_in.t1.C;
-                }
-            }
-            h.w = c.wp; h.ldw = c.ldw; h.Ktot = (int)K; h.out = bp(c.out); h.bias = c.bias; h.rowvec = c.rowvec; h.rowvec_ld = c.rowvec_ld;
-            h.residual = c.accumulate ? (const void*)bp(c.out) : (const void*)c.residual; h.base_offset_mode = 0;
-            const long long qs = conv_gn_epi(c, h.gn);
-            if (c.xfK) { h.xf_K = c.xfK; h.xf_silu = c.xf_silu; h.force_sub = 3; }
-            ++n_tc_gemms;
-            if (dry) { push(L, c.name, fl, [](cudaStream_t) { return 0; }); return qs; }
-            HaloLaunch g; int rc = build_halo(h, g);
-            if (rc) { plan_error = rc; return qs; }
-            push(L, c.name + "[halo]", fl, [g](cudaStream_t st) { return launch_halo(g, st); });
-            return qs;
-        }
-        if (c.xfK) { plan_error = fail(-31, "internal: conv '%s' was planned with a fused GroupNorm input but did not take the haloed kernel", c.name.c_str()); return -1; }
-        if (tc) {
-            ddpm_gemm_desc d; memset(&d, 0, sizeof d);
-            d.mode = GEMM_KK; d.M = (int)Pout; d.N = c.Co; d.W = c.Wo; d.H = c.Ho; d.NB = Bn;
-            d.a_ptr[0] = bp(i0); d.a_C[0] = i0.C; d.a_ld[0] = i0.C;
-            d.nseg = 1; d.seg_map[0] = 0; d.seg_taps[0] = taps; d.seg_kchunks[0] = i0.C / 64; d.seg_cbase[0] = 0;
-            if (s2) {   // SamePad2d(3,2): pad bottom/right only -> tap offsets 0..2 on the stride-2 sampled map, OOB = zero fill
-                d.a_estride = 2; d.seg_custom[0] = 1; d.seg_cmul[0] = 2;
-                for (int t = 0; t < 9; ++t) { d.seg_dx[0][t] = (signed char)(t % 3); d.seg_dy[0][t] = (signed char)(t / 3); }
-            }
-            long long K = (long long)taps * Cin;
-            if (c.has_skip) {
-                d.a_ptr[1] = bp(c.skip_in.t0); d.a_C[1] = c.skip_in.t0.C; d.a_ld[1] = c.skip_in.t0.C;
-                d.seg_map[1] = 1; d.seg_taps[1] = 1; d.seg_kchunks[1] = c.skip_in.t0.C / 64; d.seg_cbase[1] = 0; d.nseg = 2;
-                K += c.skip_in.t0.C;
-                if (c.skip_in.two) {
-                    d.a_ptr[2] = bp(c.skip_in.t1); d.a_C[2] = c.skip_in.t1.C; d.a_ld[2] = c.skip_in.t1.C;
-                    d.seg_map[2] = 2; d.seg_taps[2] = 1; d.seg_kchunks[2] = c.skip_in.t1.C / 64; d.seg_cbase[2] = 0; d.nseg = 3;
-                    K += c.skip_in.t1.C;
-                }
-            }
-            d.b_ptr = c.wp; d.b_K = (int)K; d.b_rows = c.Co; d.b_batch = 1; d.b_ld = c.ldw; d.b_bs = 0;
-            d.out = bp(c.out); d.ldo = c.Co; d.alpha = 1.f; d.grid_z = 1;
-            d.bias = c.bias; d.rowvec = c.rowvec; d.rowvec_ld = c.rowvec_ld; d.rows_per_vec = c.Ho * c.Wo;
-            d.residual = c.accumulate ? (const void*)bp(c.out) : (const void*)c.residual; d.ldr = c.Co;
-            ++n_tc_gemms;
-            // small-M problems (8x8 / 4x4 levels) do not fill the SMs with output tiles: split the K loop across CTAs
-            // (fp32 atomics into a zeroed scratch) and finish bias / timestep vector / residual / bf16 in a tiny second kernel
-            int bn = pick_block_n(c.Co);
-            int tiles = (int)((Pout + 127) / 128) * ((c.Co + bn - 1) / bn);
-            // 8x8 levels: 64 tiles of 128x256 would need split-K (+ a finalize launch and fp32 atomics); 128 tiles of 128x128
-            // fill the machine in one wave with the same MMA time per CTA and no second pass
-            static const bool no_n128 = getenv("DDPM_NO_N128_FILL") != nullptr;
-            if (!no_n128 && bn == 256 && tiles <= kPlanSms / 2 && tiles * 2 <= kPlanSms) { bn = 128; tiles *= 2; d.block_n = 128; }
-            const int slabs = (int)(K / 64);
-            int splits = 1;
-            // (a finalize launch + fp32 atomics cost more than a half-empty single wave: split only when under ~1/3 of the SMs have a tile)
-            if (tiles <= 48 && slabs >= 16) { splits = kPlanSms / tiles; if (splits > slabs / 8) splits = slabs / 8; if (splits > 16) splits = 16; if (splits < 1) splits = 1; }
-            if (splits > 1) {
-                float* scratch = at<float>(alloc_once_zero((size_t)Pout * c.Co * 4));
-                ddpm_gemm_desc ds = d;
-                ds.kk_splits = splits; ds.grid_z = splits; ds.out = scratch; ds.flags = EPI_OUT_F32 | EPI_ATOMIC;
-                ds.bias = nullptr; ds.rowvec = nullptr; ds.residual = nullptr;
-                const float* bias = c.bias; const float* rowvec = c.rowvec; const int rvld = c.rowvec_ld, rpv = c.Ho * c.Wo;
-                const bf16* resid = reinterpret_cast<const bf16*>(d.residual); bf16* outp = bp(c.out);
-                const long long M = Pout; const int N = c.Co; const int nfin = grid_for(M * (N / 8));
-                if (dry) { push(L, c.name, fl, [](cudaStream_t) { return 0; }, 2); return -1; }
-                GemmLaunch g; int rc = build_gemm(ds, g);
-                if (rc) { plan_error = rc; return -1; }
-                push(L, c.name + "[splitk]", fl, [=](cudaStream_t st) {
-                    const int r2 = launch_gemm(g, st); if (r2) return r2;
-                    launch_k(k_splitk_finalize, nfin, 256, 0, st, scratch, bias, rowvec, rvld, rpv, resid, outp, M, N);
-                    return (int)cudaGetLastError(); }, 2);
-                return -1;
-            }
-            const long long qs = conv_gn_epi(c, d.gn);
-            if (dry) { push(L, c.name, fl, [](cudaStream_t) { return 0; }); return qs; }
-            GemmLaunch g; int rc = build_gemm(d, g);
-            if (rc) { plan_error = rc; return qs; }
-            push(L, c.name, fl, [g](cudaStream_t st) { return launch_gemm(g, st); });
-            return qs;
-        }
-        ++n_generic;
-        ConvG g; memset(&g, 0, sizeof g);
-        g.in = gsrc(c.in); g.wp = c.wp; g.ldw = c.ldw; g.bias = c.bias; g.rowvec = c.rowvec; g.rowvec_ld = c.rowvec_ld;
-        g.residual = c.residual; g.out = c.out_nchw ? (void*)c.out_nchw : (void*)bp(c.out); g.out_nchw_f32 = c.out_nchw ? 1 : 0;
-        g.B = Bn; g.Hi = i0.H; g.Wi = i0.W; g.Ho = c.Ho; g.Wo = c.Wo; g.Co = c.Co; g.ksize = c.ksize; g.stride = c.stride;
-        g.pad = (c.map == MAP_NORMAL && c.stride == 1) ? c.ksize / 2 : 0; g.map = c.map; g.accumulate = c.accumulate ? 1 : 0;
-        const dim3 grid((unsigned)((Pout + 63) / 64), (unsigned)((c.Co + 63) / 64));
-        const bool nchw_dyn = c.out_nchw != nullptr;
-        UnetEngine* self = this;
-        push(L, c.name + "[simt]", fl, [g, grid, nchw_dyn, self](cudaStream_t st) {
-            ConvG gg = g; if (nchw_dyn && self->eps_dst) gg.out = self->eps_dst;
-            launch_k(k_conv_generic, grid, 256, 0, st, gg); return (int)cudaGetLastError(); });
-        if (c.has_skip) {
-            ConvG s = g; s.in = gsrc(c.skip_in); s.wp = c.wp + (long long)taps * Cin; s.ksize = 1; s.pad = 0; s.map = MAP_NORMAL; s.stride = 1;
-            s.bias = nullptr; s.rowvec = nullptr; s.residual = nullptr; s.accumulate = 1;
-            push(L, c.name + ".skip[simt]", 0, [s, grid](cudaStream_t st) { launch_k(k_conv_generic, grid, 256, 0, st, s); return (int)cudaGetLastError(); });
-        }
-        return -1;
+        static const bool no_n128 = getenv("DDPM_NO_N128_FILL") != nullptr;
+        const ConvChoice ch = conv_choose(a, !no_halo, !no_n128);
+        if (c.xfK && ch.route != CONV_ROUTE_HALO) { plan_error = fail(-31, "internal: conv '%s' was planned with a fused GroupNorm input but did not take the haloed kernel", c.name.c_str()); return -1; }
+        long long qs = -1; float* scratch = nullptr;
+        if (ch.splits > 1) scratch = at<float>(alloc_once_zero((size_t)a.B * c.Ho * c.Wo * c.Co * 4));
+        else if (ch.route != CONV_ROUTE_SIMT) { ddpm_gn_epi gn; qs = conv_gn_epi(c, gn); a.qstats = gn.qstats; }
+        ConvSteps steps;
+        const int rc = conv_fwd_steps(steps, a, ch, scratch, dry);
+        if (rc) { plan_error = rc; return qs; }
+        push_conv_steps(L, c.name, steps, flops_acc);
+        return qs;
     }
     float* eps_dst = nullptr;   // run-time destination of the final conv (caller buffer or internal eps buffer)
     PsampleEpi ps_epi = {nullptr, nullptr, nullptr, 0, nullptr};   // run-time: sampler update fused into the final gather (x != null)
@@ -572,61 +790,21 @@ struct UnetEngine {
     // weight gradient of a conv: dW (OIHW fp32, flat grads) from dy [B,Ho,Wo,Co] and the conv input
     void wgrad_op(const std::string& name, const T4& dy, const Src& in, int ksize, int stride, int map, float* dw, int Co_valid) {
         RoleScope role(this, ROLE_PARAM);
-        const int Cin = in.C(), taps = ksize * ksize, Co = dy.C;
-        const long long P = dy.pix();
-        const double fl = 2.0 * P * Co_valid * (double)taps * Cin;
-        bwd_flops += fl;
-        const bool s2 = stride == 2 && ksize == 3 && !in.two && in.t0.H == 2 * dy.H && in.t0.W == 2 * dy.W;
-        const bool tc = (stride == 1 || s2) && map == MAP_NORMAL && Co % 64 == 0 && Co == Co_valid && in.t0.C % 64 == 0 && (!in.two || in.t1.C % 64 == 0) &&
-                        tc_ok_geom(dy.H, dy.W) && (s2 || in.t0.H == dy.H);
-        if (tc) {
-            float* scratch = nullptr; size_t sc_off = 0;
-            if (taps == 9) { sc_off = alloc_once_zero((size_t)9 * Co * Cin * 4); scratch = at<float>(sc_off); }
-            for (int s = 0; s < (in.two ? 2 : 1); ++s) {
-                const T4& a = s ? in.t1 : in.t0; const int coff = s ? in.t0.C : 0;
-                ddpm_gemm_desc d; memset(&d, 0, sizeof d);
-                d.mode = GEMM_MNMN; d.M = Co; d.N = a.C; d.W = dy.W; d.H = dy.H; d.NB = dy.B;
-                d.a_ptr[0] = bp(dy); d.a_C[0] = Co; d.a_ld[0] = Co;
-                d.b_ptr = bp(a); d.b_K = a.C; d.b_ld = a.C;
-                if (s2) { d.b_estride = 2; d.b_pad = 0; }
-                d.taps = taps; d.kblocks = (int)((P + 63) / 64);
-                const int bn = pick_block_n(a.C);
-                const int tiles = ((Co + 127) / 128) * (a.C / bn) * taps;
-                // split-K so that the launch is ONE full wave (<= kPlanSms CTAs): more splits only add epilogue atomics,
-                // and kPlanSms*k + 1 CTAs would cost a whole extra wave
-                // (1x1 weight gradients are a few output tiles and HBM-bound: half a wave leaves the other SMs to the main chain)
-                int splits = ((taps == 1 && tiles <= 12) ? kPlanSms / 2 : kPlanSms) / tiles; if (splits > d.kblocks / 4) splits = d.kblocks / 4; if (splits < 1) splits = 1;
-                d.splits = splits; d.grid_z = taps * splits;
-                d.flags = EPI_OUT_F32 | EPI_ATOMIC; d.alpha = 1.f;
-                if (taps == 9) { d.out = scratch + coff; d.ldo = Cin; d.out_tap_stride = (long long)Co * Cin; }
-                else { d.out = dw + coff; d.ldo = Cin; }
-                ++n_tc_gemms;
-                // weight gradients are leaves of the backward graph: run them on the side stream, where the tensor-bound GEMMs
-                // overlap the memory-bound GroupNorm kernels of the main chain (DDPM_WGRAD_MAIN=1 keeps them in line)
-                static const bool wg_side = getenv("DDPM_WGRAD_MAIN") == nullptr;
-                if (dry) { push(bwd_ops, name, s ? 0 : fl, [](cudaStream_t) { return 0; }, 1, wg_side); continue; }
-                GemmLaunch g; int rc = build_gemm(d, g);
-                if (rc) { plan_error = rc; return; }
-                push(bwd_ops, name, s ? 0 : fl, [g](cudaStream_t st) { return launch_gemm(g, st); }, 1, wg_side);
-            }
-            if (taps == 9) {   // packed [tap][Co][Ci] scratch -> OIHW flat gradient: batched into ONE table-driven launch at the end of backward
-                PackEntry e; memset(&e, 0, sizeof e);
-                e.kind = PK_UNPACK_GRAD; e.Co = Co; e.Ci = Cin; e.taps = 9; e.fout = dw; e.scratch = scratch;
-                unpack_table_host.push_back(e);
-            }
-            return;
-        }
-        ++n_generic;
-        WgradG w; memset(&w, 0, sizeof w);
-        w.dy = bp(dy); w.in = gsrc(in); w.dw = dw; w.s_co = (long long)Cin * taps; w.s_ci = taps; w.s_tap = 1;
-        w.B = dy.B; w.Hi = in.t0.H; w.Wi = in.t0.W; w.Ho = dy.H; w.Wo = dy.W; w.Co = Co; w.ksize = ksize; w.stride = stride;
-        w.pad = (map == MAP_NORMAL && stride == 1) ? ksize / 2 : 0; w.map = map; w.Co_valid = Co_valid;
-        const int tiles = ((Cin + 63) / 64) * ((Co + 63) / 64) * taps;
-        int splits = (592 + tiles - 1) / tiles; const int maxs = (int)((P + 255) / 256); if (splits > maxs) splits = maxs; if (splits < 1) splits = 1;
-        w.pix_per_split = (int)(((P + splits - 1) / splits + 15) / 16 * 16);
-        splits = (int)((P + w.pix_per_split - 1) / w.pix_per_split);
-        const dim3 grid((Cin + 63) / 64, (Co + 63) / 64, taps * splits);
-        push(bwd_ops, name + "[simt]", fl, [w, grid](cudaStream_t st) { launch_k(k_wgrad_generic, grid, 256, 0, st, w); return (int)cudaGetLastError(); }, 1, true);
+        WgradArgs w;
+        w.dy = bp(dy); w.B = dy.B; w.Ho = dy.H; w.Wo = dy.W; w.Co = dy.C; w.Co_valid = Co_valid;
+        w.in = gsrc(in); w.Hi = in.t0.H; w.Wi = in.t0.W; w.ksize = ksize; w.stride = stride; w.map = map; w.dw = dw;
+        const bool tc = wgrad_route_tc(w);
+        // 3x3 on the tensor cores: packed [tap][Co][Ci] scratch -> OIHW flat gradient, batched into ONE table-driven launch at the
+        // end of backward
+        float* scratch = (tc && ksize == 3) ? at<float>(alloc_once_zero((size_t)9 * w.Co * w.Cin() * 4)) : nullptr;
+        ConvSteps steps; PackEntry unpack;
+        const int rc = wgrad_steps(steps, w, scratch, &unpack, dry);
+        if (rc) { plan_error = rc; return; }
+        // weight gradients are leaves of the backward graph: run them on the side stream, where the tensor-bound GEMMs
+        // overlap the memory-bound GroupNorm kernels of the main chain (DDPM_WGRAD_MAIN=1 keeps the tensor-core ones in line)
+        static const bool wg_side = getenv("DDPM_WGRAD_MAIN") == nullptr;
+        push_conv_steps(bwd_ops, name, steps, &bwd_flops, tc ? wg_side : true);
+        if (scratch) unpack_table_host.push_back(unpack);
     }
     size_t alloc_once_zero(size_t bytes) {   // carve from the plan-time-zeroed arena (contiguous region grown on demand)
         const size_t o = alloc(bytes);
@@ -720,29 +898,15 @@ struct UnetEngine {
         Packed pk; pk.ld_f = (long long)taps * Ci + extra_k;
         pk.fwd = at<bf16>(alloc((size_t)Co * pk.ld_f * 2));
         if (want_dgrad && train) { pk.ld_d = (long long)taps * Co; pk.dgr = at<bf16>(alloc((size_t)Ci * pk.ld_d * 2)); }
-        PackEntry e; memset(&e, 0, sizeof e);
-        e.kind = PK_CONV; e.Co = Co; e.Ci = Ci; e.taps = taps; e.k_off = 0; e.w = PP(pname + ".weight");
-        e.fwd = pk.fwd; e.ld_f = pk.ld_f; e.dgr = pk.dgr; e.ld_d = pk.ld_d;
-        e.dkind = pk.dgr ? (dkind_override ? dkind_override : (flip ? 2 : 1)) : 0;
-        pack_table_host.push_back(e);
+        pack_table_host.push_back(pack_conv_entry(PP(pname + ".weight"), Co, Ci, taps, 0, pk.fwd, pk.ld_f, pk.dgr, pk.ld_d,
+                                                  dkind_override ? dkind_override : (flip ? 2 : 1)));
         return pk;
     }
     void pack_extra(const std::string& pname, const Packed& into, int k_off, int Co, int Ci, bf16* dgr, long long ld_d) {
-        PackEntry e; memset(&e, 0, sizeof e);
-        e.kind = PK_CONV; e.Co = Co; e.Ci = Ci; e.taps = 1; e.k_off = k_off; e.w = PP(pname + ".weight");
-        e.fwd = into.fwd; e.ld_f = into.ld_f; e.dgr = dgr; e.ld_d = ld_d; e.dkind = dgr ? 1 : 0;
-        pack_table_host.push_back(e);
+        pack_table_host.push_back(pack_conv_entry(PP(pname + ".weight"), Co, Ci, 1, k_off, into.fwd, into.ld_f, dgr, ld_d, 1));
     }
-    void pack_identity(const Packed& into, int k_off, int C) {
-        PackEntry e; memset(&e, 0, sizeof e);
-        e.kind = PK_IDENTITY; e.Co = C; e.Ci = C; e.taps = 1; e.k_off = k_off; e.fwd = into.fwd; e.ld_f = into.ld_f;
-        pack_table_host.push_back(e);
-    }
-    void pack_bias_add(float* dst, const float* a, const float* b, int n) {
-        PackEntry e; memset(&e, 0, sizeof e);
-        e.kind = PK_BIAS_ADD; e.Co = n; e.Ci = 1; e.taps = 1; e.w = a; e.w2 = b; e.fout = dst;
-        pack_table_host.push_back(e);
-    }
+    void pack_identity(const Packed& into, int k_off, int C) { pack_table_host.push_back(pack_identity_entry(into.fwd, into.ld_f, k_off, C)); }
+    void pack_bias_add(float* dst, const float* a, const float* b, int n) { pack_table_host.push_back(pack_bias_add_entry(dst, a, b, n)); }
 
     // ------------------------------------------------------------------ blocks
     T4 res_block(const std::string& p, const Src& x, int cout, int tp_off, int tp_ld, float* TP, float* dTP);

@@ -158,7 +158,7 @@ inline T4 UnetEngine::attn_block(const std::string& p, const T4& x) {
 // output-parity sub-convolutions over dY (4+2+2+1 taps) whose epilogues scatter to the (2y+py, 2x+px) pixels.
 inline T4 UnetEngine::down_conv(const std::string& p, const T4& x) {
     const int C = x.C, Bn = x.B, h = x.H, w = x.W;
-    const bool tc = (C % 64 == 0) && tc_ok_geom(h / 2, w / 2);
+    const bool tc = conv_s2_dgrad_tc(C, h, w);
     const Packed pk = pack_conv(p, C, C, 3, 0, /*flip=*/false, true, tc ? 3 : 1);
     T4 out = newT(Bn, h / 2, w / 2, C);
     { ConvSpec c; c.name = p; c.in = one(x); c.stride = 2; c.wp = pk.fwd; c.ldw = pk.ld_f; c.bias = PP(p + ".bias"); c.out = out; c.Co = C; c.Ho = h / 2; c.Wo = w / 2;
@@ -169,31 +169,10 @@ inline T4 UnetEngine::down_conv(const std::string& p, const T4& x) {
         colsum_op(p + ".bias", dY, nullptr, 0, GP(p + ".bias"), nullptr, C);
         bool first = true; const T4 dx = grad_of(x, &first);
         if (tc) {
-            const double fl = 2.0 * dY.pix() * C * 9.0 * C;
-            bwd_flops += fl;
-            int q = 0;
-            for (int py = 0; py < 2; ++py) for (int px = 0; px < 2; ++px, ++q) {
-                ddpm_gemm_desc d; memset(&d, 0, sizeof d);
-                d.mode = GEMM_KK; d.M = (int)dY.pix(); d.N = C; d.W = w / 2; d.H = h / 2; d.NB = Bn;
-                d.a_ptr[0] = bp(dY); d.a_C[0] = C; d.a_ld[0] = C;
-                d.nseg = 1; d.seg_map[0] = 0; d.seg_kchunks[0] = C / 64; d.seg_cbase[0] = 0; d.seg_custom[0] = 1; d.seg_cmul[0] = 1;
-                int nt = 0;
-                for (int ky = py ? 1 : 0; ky < 3; ky += 2) for (int kx = px ? 1 : 0; kx < 3; kx += 2) {
-                    d.seg_dy[0][nt] = (signed char)(-(ky / 2)); d.seg_dx[0][nt] = (signed char)(-(kx / 2)); ++nt;
-                    if (px) break;
-                }
-                // (the loops above enumerate ky in {0,2} or {1} and kx in {0,2} or {1}, kx fastest)
-                d.seg_taps[0] = nt;
-                d.b_ptr = pk.dgr; d.b_K = 9 * C; d.b_rows = C; d.b_batch = 1; d.b_ld = pk.ld_d;
-                d.b_k_base = (py == 0 ? (px == 0 ? 0 : 4) : (px == 0 ? 6 : 8)) * C;
-                d.out = bp(dx); d.ldo = C; d.alpha = 1.f; d.grid_z = 1; d.o_mul = 2; d.o_py = py; d.o_px = px;
-                if (!first) { d.residual = bp(dx); d.ldr = C; }
-                ++n_tc_gemms;
-                if (dry) { push(bwd_ops, p + ".dgrad", q ? 0 : fl, [](cudaStream_t) { return 0; }); continue; }
-                GemmLaunch g; const int rc = build_gemm(d, g);
-                if (rc) { plan_error = rc; return; }
-                push(bwd_ops, p + ".dgrad", q ? 0 : fl, [g](cudaStream_t st) { return launch_gemm(g, st); });
-            }
+            ConvSteps steps;
+            const int rc = conv_s2_dgrad_steps(steps, bp(dY), Bn, h, w, C, pk.dgr, pk.ld_d, bp(dx), !first, dry);
+            if (rc) { plan_error = rc; return; }
+            push_conv_steps(bwd_ops, p + ".dgrad", steps, &bwd_flops);
         } else {
             ConvSpec c; c.name = p + ".dgrad"; c.in = one(dY); c.map = MAP_TRANSPOSED2; c.wp = pk.dgr; c.ldw = pk.ld_d; c.out = dx; c.Co = C; c.Ho = h; c.Wo = w; c.accumulate = !first;
             conv_op(bwd_ops, c, &bwd_flops);
@@ -209,37 +188,20 @@ inline T4 UnetEngine::up_conv(const std::string& p, const T4& x) {
     static const bool no_fold = getenv("DDPM_NO_UPFOLD") != nullptr;
     // (128-channel layers keep the explicit form: their folded GEMMs have 128-wide tiles, which the shared-memory operand
     // bandwidth caps below the MMA rate, so the haloed kernel on the 2x grid is used for them)
-    if (!train && !no_fold && C % 256 == 0 && tc_ok_geom(h, w)) {
+    if (!train && !no_fold && conv_fold_ok(C, h, w)) {
         // Inference plans: the upsampled tensor is never materialised.  Four output-parity sub-convolutions with 2x2 taps over the
         // low-resolution input (merged weights, PK_UPFOLD) scatter to the (2y+py, 2x+px) pixels: 4/9 of the MACs, no 2x copy.
         // (Training keeps the explicit form: the weight gradient wants the upsampled tensor as its operand.)
         Packed pk; pk.ld_f = 16LL * C; pk.fwd = at<bf16>(alloc((size_t)C * pk.ld_f * 2));
-        { PackEntry e; memset(&e, 0, sizeof e); e.kind = PK_UPFOLD; e.Co = C; e.Ci = C; e.taps = 9; e.w = PP(p + ".weight"); e.fwd = pk.fwd; e.ld_f = pk.ld_f;
-          pack_table_host.push_back(e); }
+        pack_table_host.push_back(pack_upfold_entry(PP(p + ".weight"), C, pk.fwd, pk.ld_f));
         T4 out = newT(Bn, 2 * h, 2 * w, C);
-        const double fl = 2.0 * out.pix() * C * 9.0 * C;       // the reference's count (the folded form does 4/9 of it)
-        fwd_flops += fl;
-        ddpm_gn_epi gn; memset(&gn, 0, sizeof gn);
+        double* qs = nullptr;
         static const bool no_fuse = getenv("DDPM_NO_GN_EPI") != nullptr;
-        if (!no_fuse && C % 32 == 0 && (h * w) % 32 == 0) { out.qs = (long long)zero_fwd((size_t)Bn * (C / 4) * 2 * 8); gn.qstats = at<double>((size_t)out.qs); }
-        for (int q = 0; q < 4; ++q) {
-            const int py = q >> 1, px = q & 1;
-            ddpm_gemm_desc d; memset(&d, 0, sizeof d);
-            d.mode = GEMM_KK; d.M = (int)x.pix(); d.N = C; d.W = w; d.H = h; d.NB = Bn;
-            d.a_ptr[0] = bp(x); d.a_C[0] = C; d.a_ld[0] = C;
-            d.nseg = 1; d.seg_map[0] = 0; d.seg_kchunks[0] = C / 64; d.seg_cbase[0] = 0; d.seg_custom[0] = 1; d.seg_cmul[0] = 1; d.seg_taps[0] = 4;
-            for (int a = 0; a < 2; ++a) for (int b = 0; b < 2; ++b) {
-                d.seg_dy[0][a * 2 + b] = (signed char)(py == 0 ? a - 1 : a); d.seg_dx[0][a * 2 + b] = (signed char)(px == 0 ? b - 1 : b);
-            }
-            d.b_ptr = pk.fwd; d.b_K = 16 * C; d.b_rows = C; d.b_batch = 1; d.b_ld = pk.ld_f; d.b_k_base = q * 4 * C;
-            d.out = bp(out); d.ldo = C; d.alpha = 1.f; d.grid_z = 1; d.o_mul = 2; d.o_py = py; d.o_px = px;
-            d.bias = PP(p + ".bias"); d.gn = gn;
-            ++n_tc_gemms;
-            if (dry) { push(fwd_ops, p + "[fold]", q ? 0 : fl, [](cudaStream_t) { return 0; }); continue; }
-            GemmLaunch g; const int rc = build_gemm(d, g);
-            if (rc) { plan_error = rc; return out; }
-            push(fwd_ops, p + "[fold]", q ? 0 : fl, [g](cudaStream_t st) { return launch_gemm(g, st); });
-        }
+        if (!no_fuse && C % 32 == 0 && (h * w) % 32 == 0) { out.qs = (long long)zero_fwd((size_t)Bn * (C / 4) * 2 * 8); qs = at<double>((size_t)out.qs); }
+        ConvSteps steps;
+        const int rc = conv_fold_steps(steps, bp(x), Bn, h, w, C, pk.fwd, pk.ld_f, PP(p + ".bias"), bp(out), qs, dry);
+        if (rc) { plan_error = rc; return out; }
+        push_conv_steps(fwd_ops, p, steps, &fwd_flops);
         return out;
     }
     T4 up = newT(Bn, 2 * h, 2 * w, C);

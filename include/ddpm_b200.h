@@ -131,6 +131,57 @@ int ddpm_attention_fwd_run(const ddpm_attn_desc* d, void* stream);
 int ddpm_attention_bwd_run(const ddpm_attn_bwd_desc* d, void* stream);
 long long ddpm_attn_scratch_bytes(int route, int NB, int T, int C, int backward);
 
+/* Low-level operator: one convolution of the UNet (unet.py:63-89,163-170,199-202: conv1, conv2 + skip, project_in / _out, the
+ * resample convs), its data gradient or its weight gradient, on an explicit route, with the launch steps, descriptors and packed
+ * weight layouts the UNet engine's plans use (used by the parity tests of the engine itself).
+ *  op 0  forward:         out bf16 NHWC [B][Ho][Wo][Co] = conv(x) [+ 1x1 skip(s)] + bias (+ skip_bias) + rowvec[b] + residual
+ *                         (accumulate != 0: out += instead of the residual)
+ *  op 1  data gradient:   out = dx bf16 [B][H][W][Cin0] (=, or += with accumulate) from dy bf16 [B][Ho][Wo][Co] and the same weights
+ *  op 2  weight gradient: out = dW fp32 OIHW [Co][Cin0 + Cin1][k][k] from dy and the conv input x0 | x1.  The tensor-core 1x1 and
+ *                         the CUDA-core routes ADD into out (the engine's flat gradient buffer is zeroed per backward); the
+ *                         tensor-core 3x3 routes write it.
+ * Geometry: B, H, W of the conv input; ksize 1 or 3; stride 1 (pad ksize/2) or 2 (3x3, SamePad2d: bottom / right only, H and W
+ * even, Cin0 = Co); upsample = 1 (route 5 only): nearest-2x upsample, then the 3x3 conv on the 2H x 2W grid, Cin0 = Co.
+ * Output map Ho x Wo = H x W, H/2 x W/2 (stride 2) or 2H x 2W (upsample).
+ * Inputs: x0 | x1 the channel concat [B][H][W][Cin0 | Cin1] (Cin1 = 0: one source; op 1 takes none); s0 | s1 [B][H][W][Cs0 | Cs1]
+ * the fused 1x1 skip's concat (forward of a 3x3 stride-1 conv only), or identity_skip = 1: s0 with Cs0 = Co enters with identity
+ * weights (the ResidualBlock's residual as extra K chunks).  All channel counts are multiples of 8.
+ * Weights: fp32 OIHW masters w [Co][Cin0 + Cin1][k][k] and w_skip [Co][Cs0 + Cs1], packed to bf16 by the engine's pack rows
+ * (k_pack_table) inside the call; bias / skip_bias [Co] (skip_bias with a 1x1 skip: added to bias by PK_BIAS_ADD); rowvec
+ * [B][rowvec_ld]; residual bf16 like out.  qstats (optional) [B][Co/4][2] fp64 {sum, sum of squares} per image and channel quad of
+ * the output, added to (the caller zeroes it): forward on routes 1, 2 and 4 without split-K, and route 5, with Co % 32 == 0 and
+ * a pixel count per image (route 5: of the low-resolution input) that is a multiple of 32.
+ * Routes, refused unless the engine's planner takes that route for the shape (route 2 as it does with the haloed kernel off):
+ *  1 halo: conv_halo.cuh (3x3 stride 1, H % 16 == 0, W % 8 == 0, H >= 16)
+ *  2 GEMM on the tensor cores, split over K (+ k_splitk_finalize) exactly when the planner splits; weight gradients GEMM_MNMN
+ *  3 CUDA cores: k_conv_generic (+ one launch for a skip; MAP_TRANSPOSED2 for the stride-2 data gradient), k_wgrad_generic
+ *  4 stride 2 on the tensor cores: the forward, the data gradient as four output-parity GEMMs, the weight gradient
+ *  5 nearest-2x upsample folded into the 3x3 conv: four output-parity GEMMs over merged weights (forward only)
+ * scratch: caller-owned device area of ddpm_conv_scratch_bytes(d) bytes whose first zero_bytes (see the report) must be zero on entry
+ * and are zero again on return; the rest holds the packed weights and pack table.  Buffers are 16-byte aligned.
+ * report (optional): what the call launches (route, kernel launches, block_n of the output tiles, split count over K of the
+ * tensor-core GEMM routes).  dry = 1 fills the report and does no device work.  Every argument error is refused before any device
+ * work. */
+typedef struct ddpm_conv_report {
+    int route, launches, block_n, splits;
+    long long zero_bytes;
+} ddpm_conv_report;
+typedef struct ddpm_conv_desc {
+    int op, route;
+    int B, H, W, ksize, stride, upsample;
+    int Cin0, Cin1, Co, Cs0, Cs1, identity_skip;
+    const void* x0; const void* x1; const void* s0; const void* s1; const void* dy;
+    const float* w; const float* w_skip;
+    const float* bias; const float* skip_bias; const float* rowvec; int rowvec_ld;
+    const void* residual; int accumulate;
+    void* out; double* qstats;
+    void* scratch;
+    int dry;
+    ddpm_conv_report* report;
+} ddpm_conv_desc;
+int ddpm_conv_run(const ddpm_conv_desc* d, void* stream);
+long long ddpm_conv_scratch_bytes(const ddpm_conv_desc* d);
+
 /* ------------------------------------------------------------------------------------------------
  * Low-level operators: GroupNorm(32, C, eps=1e-6) [+ SiLU] [+ dropout] (unet.py:18-20,83-84) and the bias column sums, with the
  * launch geometry the UNet engine's plans use (used by the parity tests of the engine itself).
