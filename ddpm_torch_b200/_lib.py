@@ -181,6 +181,10 @@ def lib():
             "ddpm_unet_launch_counts": ([vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)], i32),
             "ddpm_opt_step": ([vp, vp, vp, vp, vp, i64, C.POINTER(OptCfg), vp, vp, vp], i32),
             "ddpm_to_uint8_nhwc": ([vp, vp, i32, i32, i32, i32, vp], i32),
+            "ddpm_unet_temb_layout": ([vp, i32, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32),
+                                       C.POINTER(i32), C.POINTER(i32), C.POINTER(C.c_char_p)], i32),
+            "ddpm_unet_temb_forward": ([vp, vp, i32, vp, vp, vp, vp, vp], i32),
+            "ddpm_unet_temb_backward": ([vp, vp, vp, vp, vp], i32),
         }
         for name, (args, res) in sig.items():
             fn = getattr(L, name)
@@ -198,7 +202,8 @@ EXPORTS = ["ddpm_last_error", "ddpm_runtime_check", "ddpm_device_error_flag", "d
            "ddpm_unet_forward", "ddpm_unet_backward", "ddpm_unet_backward_ex", "ddpm_unet_backward_launches", "ddpm_train_forward", "ddpm_train_backward",
            "ddpm_sampler_setup", "ddpm_sampler_reset", "ddpm_sampler_step", "ddpm_sampler_step_pred",
            "ddpm_bpd_setup", "ddpm_bpd_reset", "ddpm_bpd_step", "ddpm_unet_grad_chunks", "ddpm_unet_wait_grad_chunk", "ddpm_unet_plan_stats",
-           "ddpm_unet_launches_per_forward", "ddpm_unet_launch_counts", "ddpm_opt_step", "ddpm_to_uint8_nhwc"]
+           "ddpm_unet_launches_per_forward", "ddpm_unet_launch_counts", "ddpm_opt_step", "ddpm_to_uint8_nhwc",
+           "ddpm_unet_temb_layout", "ddpm_unet_temb_forward", "ddpm_unet_temb_backward"]
 
 
 def check(rc, what=""):

@@ -16,6 +16,8 @@ struct ddpm_unet {
     // t_model i64[T] = 0..T-1, rows f32[T][kBpdRow], sqrt_ab f32[T], sqrt_1mab f32[T]
     void* d_bpd = nullptr; int bpd_T = 0;
     const float* train_target = nullptr;
+    bool temb_rows = false;        // the last forward of this plan was a per-row ddpm_unet_temb_forward (what its backward reads);
+                                   // every other forward entry point clears it
 };
 
 __global__ void k_set_int(int* p, int v) {
@@ -481,7 +483,7 @@ int ddpm_unet_plan(ddpm_unet* h, int B, int H, int W, int training, float* param
     if (!params_flat || !workspace) return fail(-30, "params / workspace pointer is null");
     if (training && !grads_flat) return fail(-30, "training plan needs a gradient buffer");
     int rc = ddpm_runtime_check(); if (rc) return rc;
-    e.planned = false;
+    e.planned = false; h->temb_rows = false;
     e.P = params_flat; e.G = grads_flat; e.ws = static_cast<uint8_t*>(workspace); e.ws_bytes = (size_t)workspace_bytes;
     e.zf_cursor = e.zb_cursor = 0;
     if ((rc = e.plan(B, H, W, training != 0, true))) return rc;
@@ -498,6 +500,7 @@ int ddpm_unet_repack(ddpm_unet* h, void* stream) { NEED_PLAN(h); return h->e.rep
 int ddpm_unet_forward(ddpm_unet* h, const float* x, const int64_t* t, float* eps, uint64_t dropout_seed, void* stream) {
     NEED_PLAN(h);
     UnetEngine& e = h->e;
+    h->temb_rows = false;
     e.x_in = x; e.t_in = reinterpret_cast<const long long*>(t); e.eps_dst = eps; e.drop_seed = dropout_seed;
     return e.run_list(e.fwd_ops, static_cast<cudaStream_t>(stream));
 }
@@ -527,6 +530,7 @@ int ddpm_train_forward(ddpm_unet* h, const float* x0, const int64_t* t, const fl
     if (h && h->e.cfg.in_channels != h->e.cfg.out_channels) return fail(-30, "ddpm_train_forward: eps prediction needs out_channels == in_channels");
     NEED_PLAN(h);
     UnetEngine& e = h->e;
+    h->temb_rows = false;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int per_img = e.cfg.in_channels * e.H * e.W;
     const long long total = (long long)e.B * per_img;
@@ -587,6 +591,7 @@ int ddpm_sampler_step_pred(ddpm_unet* h, float* x, const float* z, uint64_t seed
     NEED_PLAN(h);
     if (!h->d_coef) return fail(-33, "ddpm_sampler_setup has not been called");
     UnetEngine& e = h->e;
+    h->temb_rows = false;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     long long* tbuf = e.at<long long>(e.tbuf_off); float* cc = e.at<float>(e.coefcur_off); float* eps = e.at<float>(e.eps_off);
     launch_k(k_sampler_prep, 1, 256, 0, st, e.at<int>(e.counter_off), h->d_tmodel, h->d_coef, 6, tbuf, cc, e.B);
@@ -645,6 +650,7 @@ int ddpm_bpd_step(ddpm_unet* h, const float* x0, const float* noise, int clip_de
     NEED_PLAN(h);
     if (!h->d_bpd) return fail(-33, "ddpm_bpd_setup has not been called");
     UnetEngine& e = h->e;
+    h->temb_rows = false;
     const int Cin = e.cfg.in_channels, Cout = e.cfg.out_channels, HW = e.H * e.W, T = h->bpd_T;
     if (Cin != Cout) return fail(-30, "ddpm_bpd_step: eps prediction needs out_channels == in_channels");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -752,6 +758,79 @@ int ddpm_unet_launch_counts(const ddpm_unet* h, int* fwd, int* bwd, int* pack) {
     if (fwd) *fwd = UnetEngine::count_launches(h->e.fwd_ops);
     if (bwd) *bwd = h->e.count_bwd_launches(false, true);     // the default backward (no dx)
     if (pack) *pack = UnetEngine::count_launches(h->e.pack_ops);
+    return 0;
+}
+
+// ------------------------------------------------------------------------------------------------ timestep-path probes
+int ddpm_unet_temb_layout(const ddpm_unet* h, int max_n, int* route, int* has_uniform, int* E, int* tp_ld, int* maxc,
+                          int* off, int* cout, const char** block) {
+    if (!h) return fail(-30, "ddpm_unet_temb_layout: null handle");
+    const UnetEngine& e = h->e;
+    if (e.temb.E <= 0) return fail(-33, "ddpm_unet_temb_layout: no plan (ddpm_unet_workspace_bytes or ddpm_unet_plan first)");
+    if (route) *route = e.temb.tc ? 1 : 0;
+    if (has_uniform) *has_uniform = e.temb_uni_ops.empty() ? 0 : 1;
+    if (E) *E = e.temb.E;
+    if (tp_ld) *tp_ld = e.temb.tp_ld;
+    if (maxc) *maxc = e.temb.maxc;
+    const int n = (int)e.fc_table_host.size();
+    for (int i = 0; i < n && i < max_n; ++i) {
+        if (off) off[i] = e.fc_table_host[i].off;
+        if (cout) cout[i] = e.fc_table_host[i].cout;
+        if (block) block[i] = e.tp_block_host[i].c_str();
+    }
+    return n;
+}
+
+int ddpm_unet_temb_forward(ddpm_unet* h, const int64_t* t, int uniform, float* emb, float* e0, float* e1, float* tp, void* stream) {
+    if (!h) return fail(-30, "ddpm_unet_temb_forward: null handle");
+    if (!t) return fail(-30, "ddpm_unet_temb_forward: null t");
+    if (uniform != 0 && uniform != 1) return fail(-30, "ddpm_unet_temb_forward: uniform must be 0 or 1 (got %d)", uniform);
+    NEED_PLAN(h);
+    UnetEngine& e = h->e;
+    if (uniform && e.temb_uni_ops.empty()) return fail(-30, "ddpm_unet_temb_forward: this plan has no one-row timestep route");
+    // the forward's own zero op, then its timestep ops, or the one-row ops run_list swaps in for them under uniform_t
+    std::vector<Op> ops;
+    for (const Op& o : e.fwd_ops) if (o.name == "zero.fwd") ops.push_back(o);
+    if (ops.size() != 1) return fail(-31, "ddpm_unet_temb_forward: internal: the plan has no 'zero.fwd' op");
+    if (uniform) ops.insert(ops.end(), e.temb_uni_ops.begin(), e.temb_uni_ops.end());
+    else for (const Op& o : e.fwd_ops) if (o.tag == OP_TEMB) ops.push_back(o);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    h->temb_rows = false;
+    e.t_in = reinterpret_cast<const long long*>(t);
+    int rc = e.run_list(ops, st);           // honours Op::wait_pack: the tensor-core projection waits for a pending repack
+    if (rc) return rc;
+    const size_t Bn = (size_t)e.B, E_ = (size_t)e.temb.E;
+    const struct { float* dst; const float* src; size_t n; } cp[] = {
+        {emb, e.temb.emb, Bn * e.cfg.hid_channels}, {e0, e.temb.e0, Bn * E_}, {e1, e.temb.e1, Bn * E_}, {tp, e.temb.TP, Bn * e.temb.tp_ld}};
+    for (const auto& c : cp)
+        if (c.dst) DDPM_CUDA_OK(cudaMemcpyAsync(c.dst, c.src, c.n * 4, cudaMemcpyDefault, st));
+    h->temb_rows = !uniform;
+    return 0;
+}
+
+int ddpm_unet_temb_backward(ddpm_unet* h, const float* dtp, float* d_st, float* d_s0, void* stream) {
+    if (!h) return fail(-30, "ddpm_unet_temb_backward: null handle");
+    if (!dtp) return fail(-30, "ddpm_unet_temb_backward: null dTP");
+    NEED_PLAN(h);
+    UnetEngine& e = h->e;
+    if (!e.train) return fail(-33, "ddpm_unet_temb_backward: plan was built without training");
+    if (!h->temb_rows) return fail(-33, "ddpm_unet_temb_backward: needs a per-row ddpm_unet_temb_forward (uniform = 0) of this plan first");
+    // the backward's zero op (accumulators + the flat gradient buffer), dTP in place of what the ResBlocks deposit, then the
+    // timestep ops of the backward list
+    std::vector<Op> zero, ops;
+    for (const Op& o : e.bwd_ops) {
+        if (o.name == "zero.bwd") zero.push_back(o);
+        if (o.name == "temb.dtp_cast" || o.name == "temb.proj.bwd" || o.name == "temb.mlp.bwd") ops.push_back(o);
+    }
+    if (zero.size() != 1 || ops.size() != (e.temb.tc ? 3u : 2u)) return fail(-31, "ddpm_unet_temb_backward: internal: timestep ops not found");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    e.bwd_params = true;
+    int rc = e.run_list(zero, st);
+    if (rc) return rc;
+    DDPM_CUDA_OK(cudaMemcpyAsync(e.temb.dTP, dtp, (size_t)e.B * e.temb.tp_ld * 4, cudaMemcpyDefault, st));
+    if ((rc = e.run_list(ops, st))) return rc;
+    if (d_st) DDPM_CUDA_OK(cudaMemcpyAsync(d_st, e.temb.d_st, (size_t)e.B * e.temb.E * 4, cudaMemcpyDefault, st));
+    if (d_s0) DDPM_CUDA_OK(cudaMemcpyAsync(d_s0, e.temb.d_s0, (size_t)e.B * e.temb.E * 4, cudaMemcpyDefault, st));
     return 0;
 }
 

@@ -589,6 +589,10 @@ struct UnetEngine {
     std::vector<FcEnt> fc_table_host; size_t fc_table_off = 0;   // tensor-core timestep projections (concatenated fc weights)
     bool uniform_t = false;                // set by ddpm_sampler_step around its forward
     std::vector<SgemmParams> tpw_table_host, tpd_table_host; size_t tpw_table_off = 0, tpd_table_off = 0;
+    // the timestep path's buffers and layout as planned (read by the ddpm_unet_temb_* probes); block names in tp_entry order
+    struct TembBufs { float *emb = nullptr, *e0 = nullptr, *e1 = nullptr, *TP = nullptr, *dTP = nullptr, *d_st = nullptr, *d_s0 = nullptr;
+                      int E = 0, tp_ld = 0, maxc = 0; bool tc = false; } temb;
+    std::vector<std::string> tp_block_host;
     uint32_t layer_counter = 0;
     double fwd_flops = 0, bwd_flops = 0;
     int n_tc_gemms = 0, n_generic = 0;

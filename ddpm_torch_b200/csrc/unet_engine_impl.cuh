@@ -276,6 +276,7 @@ inline int UnetEngine::plan(int B_, int H_, int W_, bool train_, bool dry_) {
     cursor = 0; pack_ops.clear(); fwd_ops.clear(); bwd_ops.clear(); tape.clear(); tape_tag.clear(); cur_tag = "late"; grads.clear(); once_list.clear();
     { std::vector<GradChunk> keep; keep.swap(chunks); for (auto& c : keep) if (c.ev) cudaEventDestroy(c.ev); }
     tp_table_host.clear(); tp_uni_table_host.clear(); fc_table_host.clear(); tpw_table_host.clear(); tpd_table_host.clear(); pack_table_host.clear(); unpack_table_host.clear();
+    tp_block_host.clear(); temb = TembBufs{};
     layer_counter = 0; fwd_flops = bwd_flops = 0; n_tc_gemms = n_generic = 0; plan_error = 0; gather_fused_tail = false; out_T = nullptr;
     const size_t zf_total = zf_cursor, zb_total = zb_cursor;   // sizes learned by the preceding dry pass
     zf_cursor = zb_cursor = 0;
@@ -319,6 +320,8 @@ inline int UnetEngine::plan(int B_, int H_, int W_, bool train_, bool dry_) {
     bf16* WcatT = (tc_temb && train) ? at<bf16>(alloc_once_zero((size_t)tp_ld * E * 2)) : nullptr;
     float* bias_cat = tc_temb ? at<float>(alloc_once_zero((size_t)tp_ld * 4)) : nullptr;
     bf16* A_f = tc_temb ? at<bf16>(alloc((size_t)B * E * 2)) : nullptr;
+    temb.emb = emb; temb.e0 = e0; temb.e1 = e1; temb.TP = TP; temb.dTP = dTP; temb.d_st = d_st;
+    temb.E = E; temb.tp_ld = tp_ld; temb.maxc = maxc; temb.tc = tc_temb;
     const size_t temb_first = fwd_ops.size();
     {
         const int Bn = B;
@@ -383,6 +386,7 @@ inline int UnetEngine::plan(int B_, int H_, int W_, bool train_, bool dry_) {
         tp_table_host.push_back(s);
         { SgemmParams u = s; u.M = 1; tp_uni_table_host.push_back(u); }
         { FcEnt f; f.w = PP(p + ".fc.weight"); f.b = PP(p + ".fc.bias"); f.gw = train ? GP(p + ".fc.weight") : nullptr; f.cout = cout; f.off = off; fc_table_host.push_back(f); }
+        tp_block_host.push_back(p);
         fwd_flops += 2.0 * B * cout * E;
         if (train) {
             // dW_fc[o][e] = sum_b silu(e1[b][e]) * dTP[b][off+o]   (computed as C'[e][o], stored transposed)
@@ -441,6 +445,7 @@ inline int UnetEngine::plan(int B_, int H_, int W_, bool train_, bool dry_) {
             } else
             push(bwd_ops, "temb.proj.bwd", 0, [=](cudaStream_t st) { launch_k(k_sgemm_table, gw, 256, 0, st, tw, 1); launch_k(k_sgemm_table, gd, 256, 0, st, td, 1); return (int)cudaGetLastError(); }, 2);
             float* d_e1 = at<float>(alloc((size_t)B * E * 4)); float* d_s0 = at<float>(zero_bwd((size_t)B * E * 4)); float* d_e0 = at<float>(alloc((size_t)B * E * 4));
+            self->temb.d_s0 = d_s0;
             const long long nE = (long long)B * E; const int Bn = B;
             float* gw2 = GP("embed.2.weight"); float* gb2 = GP("embed.2.bias"); float* gw0 = GP("embed.0.weight"); float* gb0 = GP("embed.0.bias");
             const float* w2 = PP("embed.2.weight");

@@ -334,6 +334,22 @@ int ddpm_unet_launches_per_forward(const ddpm_unet* h);
 /* kernel launches issued by one forward / backward / repack of the compiled plan (memsets not counted) */
 int ddpm_unet_launch_counts(const ddpm_unet* h, int* fwd, int* bwd, int* pack);
 
+/* ---- timestep-path probes: run a plan's own timestep ops alone (operator-level tests of the engine).
+ * Layout of a planned (or dry-planned) handle's per-block projections TP [B][tp_ld]: route 0 = CUDA cores, 1 = tensor cores;
+ * has_uniform = the plan has the one-row route ddpm_sampler_step swaps in; block i (in the order the forward runs the ResBlocks,
+ * e.g. "downsamples.level_1.0.0") owns columns off[i] .. off[i] + cout[i] - 1 of TP, the output of its `fc`.  Fills at most max_n
+ * entries of off / cout / block (any pointer may be NULL; the names live until the next plan) and returns the block count. */
+int ddpm_unet_temb_layout(const ddpm_unet* h, int max_n, int* route, int* has_uniform, int* temb_dim, int* tp_ld, int* maxc,
+                          int* off, int* cout, const char** block);
+/* The plan's "zero.fwd" op, then its timestep ops (uniform = 1: the one-row ops + broadcast exactly as ddpm_sampler_step runs
+ * them; refused on a plan without them), waiting for a pending repack as the forward does.  Copies out (device pointers, any may
+ * be NULL) emb [B][hid], e0 = Linear(emb) [B][E], e1 = Linear(SiLU(e0)) [B][E] (row 0 only under uniform) and TP [B][tp_ld]. */
+int ddpm_unet_temb_forward(ddpm_unet* h, const int64_t* t, int uniform, float* emb, float* e0, float* e1, float* tp, void* stream);
+/* Training plans, right after a per-row ddpm_unet_temb_forward (any other forward of the plan in between is refused): the backward's "zero.bwd" op (which clears the flat gradient buffer),
+ * dtp [B][tp_ld] (device) copied into the plan's dTP, then the backward's timestep ops; the fc.weight and embed.* gradients land
+ * in the flat gradient buffer.  Copies out d_st = dL/dSiLU(e1) and d_s0 = dL/dSiLU(e0), [B][E] each (may be NULL). */
+int ddpm_unet_temb_backward(ddpm_unet* h, const float* dtp, float* d_st, float* d_s0, void* stream);
+
 /* ---- fused optimizer step over the flat fp32 buffers.
  * Replaces, per training step, nn.utils.clip_grad_norm_(params, max_norm) + Adam.step() + LambdaLR warm-up + EMA.update()
  * (utils/train.py:159-165, :300-305; train.py:128-132) = ~13 tiny kernels x 304 tensors, by two launches and no host sync.
