@@ -10,6 +10,7 @@ from . import parallel
 from . import optim
 from . import postprocess
 from . import checkpoint
+from . import metrics
 from .optim import EMA, FusedAdam
 
 __all__ = ["UNet", "GaussianDiffusion", "get_beta_schedule", "DDIM", "get_selection_schedule", "EMA", "FusedAdam", "ModelWrapper"]

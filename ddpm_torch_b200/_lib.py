@@ -185,6 +185,9 @@ def lib():
                                        C.POINTER(i32), C.POINTER(i32), C.POINTER(C.c_char_p)], i32),
             "ddpm_unet_temb_forward": ([vp, vp, i32, vp, vp, vp, vp, vp], i32),
             "ddpm_unet_temb_backward": ([vp, vp, vp, vp, vp], i32),
+            "ddpm_knn_scratch_bytes": ([i32, i32, i32, i32], i64),
+            "ddpm_knn_kth": ([vp, i32, i64, vp, i32, i64, i32, i32, vp, vp, i64, vp], i32),
+            "ddpm_knn_cover": ([vp, i32, i64, vp, i32, i64, i32, vp, vp, vp, i64, vp], i32),
         }
         for name, (args, res) in sig.items():
             fn = getattr(L, name)
@@ -203,7 +206,8 @@ EXPORTS = ["ddpm_last_error", "ddpm_runtime_check", "ddpm_device_error_flag", "d
            "ddpm_sampler_setup", "ddpm_sampler_reset", "ddpm_sampler_step", "ddpm_sampler_step_pred",
            "ddpm_bpd_setup", "ddpm_bpd_reset", "ddpm_bpd_step", "ddpm_unet_grad_chunks", "ddpm_unet_wait_grad_chunk", "ddpm_unet_plan_stats",
            "ddpm_unet_launches_per_forward", "ddpm_unet_launch_counts", "ddpm_opt_step", "ddpm_to_uint8_nhwc",
-           "ddpm_unet_temb_layout", "ddpm_unet_temb_forward", "ddpm_unet_temb_backward"]
+           "ddpm_unet_temb_layout", "ddpm_unet_temb_forward", "ddpm_unet_temb_backward",
+           "ddpm_knn_scratch_bytes", "ddpm_knn_kth", "ddpm_knn_cover"]
 
 
 def check(rc, what=""):

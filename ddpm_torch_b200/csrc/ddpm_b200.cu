@@ -5,6 +5,7 @@
 #include <initializer_list>
 #include "unet_engine_impl.cuh"
 #include "optim.cuh"
+#include "knn.cuh"
 
 using namespace ddpm;
 
@@ -428,6 +429,58 @@ int ddpm_conv_run(const ddpm_conv_desc* d, void* stream) {
         if ((e = cudaGetLastError()) != cudaSuccess) return fail(-20, "%s: gradient unpack failed: %s", fn, cudaGetErrorString(e));
     }
     return 0;
+}
+
+// ------------------------------------------------------------------------------------------------ precision / recall k-NN
+static int knn_check(const char* fn, int n_rows, int n_cols, int D, int kk) {
+    if (n_rows < 1 || n_cols < 1 || D < 1) return fail(-45, "%s: need n_rows >= 1, n_cols >= 1 and D >= 1", fn);
+    if (kk < 0 || kk > KNN_MAX_K) return fail(-45, "%s: kk = nhood_size + 1 must be in 1..%d (nhood_size <= %d), got %d", fn, KNN_MAX_K, KNN_MAX_K - 1, kk);
+    if (kk > n_cols) return fail(-45, "%s: kk = %d exceeds the %d columns", fn, kk, n_cols);
+    if (n_rows > (1 << 30) || n_cols > (1 << 30)) return fail(-45, "%s: more than 2^30 rows or columns", fn);
+    return 0;
+}
+static int knn_check_mat(const char* fn, const char* what, const void* x, long long ld, int D) {
+    if (!x) return fail(-45, "%s: null %s", fn, what);
+    if (misaligned16(x) || ld < D || ld % 8) return fail(-45, "%s: %s needs a 16-byte aligned base and a row pitch ld >= D with ld %% 8 == 0 (got ld = %lld, D = %d)", fn, what, ld, D);
+    return 0;
+}
+
+long long ddpm_knn_scratch_bytes(int n_rows, int n_cols, int D, int kk) {
+    const int rc = knn_check("ddpm_knn_scratch_bytes", n_rows, n_cols, D, kk);
+    return rc ? rc : (long long)knn_plan(n_rows, n_cols, D, kk).total;
+}
+
+// ManifoldBuilder.compute_kth (precision_recall.py:156-164): kth_out[i] = the (kk)-th smallest distance from row i to all columns.
+int ddpm_knn_kth(const void* rows, int n_rows, long long ld_rows, const void* cols, int n_cols, long long ld_cols, int D, int kk,
+                 void* kth_out, void* scratch, long long bytes, void* stream) {
+    const char* fn = "ddpm_knn_kth";
+    int rc = knn_check(fn, n_rows, n_cols, D, kk);
+    if (!rc && kk < 1) rc = fail(-45, "%s: kk must be >= 1", fn);
+    if (!rc) rc = knn_check_mat(fn, "rows", rows, ld_rows, D);
+    if (!rc) rc = knn_check_mat(fn, "cols", cols, ld_cols, D);
+    if (rc) return rc;
+    if (!kth_out) return fail(-45, "%s: null kth_out", fn);
+    const size_t need = knn_plan(n_rows, n_cols, D, kk).total;
+    if (!scratch || misaligned16(scratch) || bytes < (long long)need)
+        return fail(-45, "%s: needs a 16-byte aligned scratch of ddpm_knn_scratch_bytes = %zu bytes (got %lld)", fn, need, bytes);
+    return knn_launch(static_cast<const __half*>(rows), n_rows, ld_rows, static_cast<const __half*>(cols), n_cols, ld_cols, D, kk,
+                      nullptr, kth_out, scratch, static_cast<cudaStream_t>(stream));
+}
+
+// calc_pr (precision_recall.py:177-206), one direction: covered[i] = any_j dist(probe i, support j) <= radii[j].
+int ddpm_knn_cover(const void* probes, int n_probes, long long ld_p, const void* support, int n_support, long long ld_s, int D,
+                   const void* radii, uint8_t* covered, void* scratch, long long bytes, void* stream) {
+    const char* fn = "ddpm_knn_cover";
+    int rc = knn_check(fn, n_probes, n_support, D, 0);
+    if (!rc) rc = knn_check_mat(fn, "probes", probes, ld_p, D);
+    if (!rc) rc = knn_check_mat(fn, "support", support, ld_s, D);
+    if (rc) return rc;
+    if (!radii || !covered) return fail(-45, "%s: null radii or covered", fn);
+    const size_t need = knn_plan(n_probes, n_support, D, 0).total;
+    if (!scratch || misaligned16(scratch) || bytes < (long long)need)
+        return fail(-45, "%s: needs a 16-byte aligned scratch of ddpm_knn_scratch_bytes(.., kk = 0) = %zu bytes (got %lld)", fn, need, bytes);
+    return knn_launch(static_cast<const __half*>(probes), n_probes, ld_p, static_cast<const __half*>(support), n_support, ld_s, D, 0,
+                      static_cast<const __half*>(radii), covered, scratch, static_cast<cudaStream_t>(stream));
 }
 
 // ------------------------------------------------------------------------------------------------ UNet engine

@@ -183,6 +183,24 @@ int ddpm_conv_run(const ddpm_conv_desc* d, void* stream);
 long long ddpm_conv_scratch_bytes(const ddpm_conv_desc* d);
 
 /* ------------------------------------------------------------------------------------------------
+ * k-NN half of the improved precision/recall metric (ddpm_torch/metrics/precision_recall.py): one fp16 wgmma GEMM per pass with a
+ * selection epilogue (knn.cuh), in place of the reference's fp16 cdist blocks copied to the host.  Feature matrices are fp16
+ * [n][ld] (device), 16-byte aligned, ld >= D and ld % 8 == 0 (elements past D in a row are ignored).  Any D >= 1.
+ *   na[i] = sum_d a[i,d]^2 (fp32);  d2[i,j] = max(0, na[i] + nb[j] - 2 <a_i, b_j>) (fp16 wgmma, fp32 accumulation)
+ * ddpm_knn_kth   (compute_kth, :156-164): kth_out fp16 [n_rows] = fp16_rn(sqrt_rn(kk-th smallest d2[i, .])), all columns
+ *                including row i itself when rows == cols; kk = nhood_size + 1 in 1..16 and kk <= n_cols.
+ * ddpm_knn_cover (calc_pr, :177-206, one direction): covered u8 [n_probes] = 1 iff some support j has
+ *                fp16_rn(sqrt_rn(d2[i,j])) <= radii[j] (fp16 [n_support]), else 0.
+ * scratch: caller-owned, 16-byte aligned, ddpm_knn_scratch_bytes(n_rows, n_cols, D, kk) bytes (kk = 0 for ddpm_knn_cover); no
+ * initialisation needed.  No allocation, no synchronisation, graph-capturable; results are bit-identical from call to call.  Every
+ * argument error is refused before any device work. */
+long long ddpm_knn_scratch_bytes(int n_rows, int n_cols, int D, int kk);
+int ddpm_knn_kth(const void* rows, int n_rows, long long ld_rows, const void* cols, int n_cols, long long ld_cols, int D, int kk,
+                 void* kth_out, void* scratch, long long bytes, void* stream);
+int ddpm_knn_cover(const void* probes, int n_probes, long long ld_p, const void* support, int n_support, long long ld_s, int D,
+                   const void* radii, uint8_t* covered, void* scratch, long long bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Low-level operators: GroupNorm(32, C, eps=1e-6) [+ SiLU] [+ dropout] (unet.py:18-20,83-84) and the bias column sums, with the
  * launch geometry the UNet engine's plans use (used by the parity tests of the engine itself).
  * Input = channel concat of two NHWC bf16 sources x0 [B][HW][C0] and x1 [B][HW][C1] (C1 = 0: one source).  C0 and C1 are
