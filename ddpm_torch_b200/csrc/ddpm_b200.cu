@@ -2,10 +2,12 @@
 #include <cstdarg>
 #include <new>
 #include <cmath>
+#include <climits>
 #include <initializer_list>
 #include "unet_engine_impl.cuh"
 #include "optim.cuh"
 #include "knn.cuh"
+#include "fid.cuh"
 
 using namespace ddpm;
 
@@ -481,6 +483,62 @@ int ddpm_knn_cover(const void* probes, int n_probes, long long ld_p, const void*
         return fail(-45, "%s: needs a 16-byte aligned scratch of ddpm_knn_scratch_bytes(.., kk = 0) = %zu bytes (got %lld)", fn, need, bytes);
     return knn_launch(static_cast<const __half*>(probes), n_probes, ld_p, static_cast<const __half*>(support), n_support, ld_s, D, 0,
                       static_cast<const __half*>(radii), covered, scratch, static_cast<cudaStream_t>(stream));
+}
+
+// ------------------------------------------------------------------------------------------------ Fréchet Inception Distance
+static int fid_check_d(const char* fn, int D) {
+    if (D < 1 || D > FID_MAX_D) return fail(-46, "%s: D must be in 1..%d (got %d)", fn, FID_MAX_D, D);
+    return 0;
+}
+
+long long ddpm_fid_stats_bytes(int D) {
+    const int rc = fid_check_d("ddpm_fid_stats_bytes", D);
+    return rc ? rc : (long long)fid_stats_bytes(D);
+}
+
+long long ddpm_fid_distance_scratch_bytes(int D) {
+    const int rc = fid_check_d("ddpm_fid_distance_scratch_bytes", D);
+    return rc ? rc : (long long)fid_dist_bytes(D);
+}
+
+// InceptionStatistics.forward (fid_score.py:116-135): the batch's features stay on the device; no np.cov, no Chan merge.
+int ddpm_fid_stats_update(void* state, int D, const float* feats, long long n, long long ld, void* stream) {
+    const char* fn = "ddpm_fid_stats_update";
+    if (int rc = fid_check_d(fn, D)) return rc;
+    if (!state || misaligned16(state)) return fail(-46, "%s: state must be a non-null, 16-byte aligned buffer", fn);
+    if (n < 0 || n > INT_MAX) return fail(-46, "%s: n must be in 0..2^31-1 (got %lld)", fn, n);
+    if (n == 0) return 0;
+    if (!feats || (reinterpret_cast<uintptr_t>(feats) & 3)) return fail(-46, "%s: feats must be a non-null, 4-byte aligned fp32 buffer", fn);
+    if (ld < D) return fail(-46, "%s: row pitch ld = %lld must be >= D = %d", fn, ld, D);
+    const cudaError_t e = fid_stats_launch(state, D, feats, n, ld, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? 0 : fail(-20, "%s: launch failed: %s", fn, cudaGetErrorString(e));
+}
+
+// InceptionStatistics.get_statistics (fid_score.py:137-142, ddof = 1) and the running values (ddof = 0).
+int ddpm_fid_stats_finalize(const void* state, int D, long long n, int ddof, double* mean_out, double* cov_out, void* stream) {
+    const char* fn = "ddpm_fid_stats_finalize";
+    if (int rc = fid_check_d(fn, D)) return rc;
+    if (!state || misaligned16(state) || !mean_out || !cov_out) return fail(-46, "%s: null or misaligned state / output", fn);
+    if (ddof != 0 && ddof != 1) return fail(-46, "%s: ddof must be 0 or 1 (got %d)", fn, ddof);
+    if (n <= ddof) return fail(-46, "%s: needs n > ddof (n = %lld, ddof = %d)", fn, n, ddof);
+    const cudaError_t e = fid_finalize_launch(state, D, n, ddof, mean_out, cov_out, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? 0 : fail(-20, "%s: launch failed: %s", fn, cudaGetErrorString(e));
+}
+
+// calc_fd / calculate_frechet_distance (fid_score.py:186-187, :269-323): no sqrtm of the non-symmetric product; see fid.cuh.
+int ddpm_fid_distance(const double* mu1, const double* sigma1, const double* mu2, const double* sigma2, int D, double* out,
+                      void* scratch, long long bytes, void* stream) {
+    const char* fn = "ddpm_fid_distance";
+    if (int rc = fid_check_d(fn, D)) return rc;
+    if (!mu1 || !sigma1 || !mu2 || !sigma2 || !out) return fail(-46, "%s: null input or output", fn);
+    if ((reinterpret_cast<uintptr_t>(mu1) | reinterpret_cast<uintptr_t>(sigma1) | reinterpret_cast<uintptr_t>(mu2) |
+         reinterpret_cast<uintptr_t>(sigma2) | reinterpret_cast<uintptr_t>(out)) & 7)
+        return fail(-46, "%s: inputs and output must be 8-byte aligned fp64 buffers", fn);
+    const size_t need = fid_dist_bytes(D);
+    if (!scratch || misaligned16(scratch) || bytes < (long long)need)
+        return fail(-46, "%s: needs a 16-byte aligned scratch of ddpm_fid_distance_scratch_bytes = %zu bytes (got %lld)", fn, need, bytes);
+    const cudaError_t e = fid_distance_launch(mu1, sigma1, mu2, sigma2, D, out, scratch, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? 0 : fail(-20, "%s: launch failed: %s", fn, cudaGetErrorString(e));
 }
 
 // ------------------------------------------------------------------------------------------------ UNet engine

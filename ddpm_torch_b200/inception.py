@@ -1,0 +1,144 @@
+"""FID Inception-v3 (``ddpm_torch/metrics/inception.py``): the TensorFlow FID network, assembled from torchvision's Inception
+building blocks.  Torch only: Inception runs on torch / cuDNN; only the statistics and the distance run on the engine.
+
+The FID network differs from torchvision's ImageNet Inception-v3 in three places, all reproduced here:
+  * 1008 classes (its ``fc`` is part of the checkpoint, though no feature uses it);
+  * the 3x3 average pools inside the A, C and E blocks exclude the padding (TensorFlow's ``count_include_pad=False``);
+  * the last E block (``Mixed_7c``) pools its pool branch with a 3x3 max pool.
+Module names follow torchvision's ``Inception3``, so the published ``pt_inception-2015-12-05-6726825d.pth`` loads with
+``strict=True``, and ``InceptionV3``'s own ``state_dict`` has the reference's ``blocks.<i>.<j>`` keys.
+"""
+import os
+
+import torch
+import torch.nn as nn
+import torch.nn.functional as F
+import torchvision.models.inception as tvi
+
+FID_WEIGHTS_URL = "https://github.com/mseitzer/pytorch-fid/releases/download/fid_weights/pt_inception-2015-12-05-6726825d.pth"
+
+
+def _avg3(x):
+    return F.avg_pool2d(x, kernel_size=3, stride=1, padding=1, count_include_pad=False)
+
+
+def _max3(x):
+    return F.max_pool2d(x, kernel_size=3, stride=1, padding=1)
+
+
+class _BlockA(tvi.InceptionA):
+    def forward(self, x):
+        b5 = self.branch5x5_2(self.branch5x5_1(x))
+        b3 = self.branch3x3dbl_3(self.branch3x3dbl_2(self.branch3x3dbl_1(x)))
+        return torch.cat([self.branch1x1(x), b5, b3, self.branch_pool(_avg3(x))], 1)
+
+
+class _BlockC(tvi.InceptionC):
+    def forward(self, x):
+        b7 = self.branch7x7_3(self.branch7x7_2(self.branch7x7_1(x)))
+        d = x
+        for m in (self.branch7x7dbl_1, self.branch7x7dbl_2, self.branch7x7dbl_3, self.branch7x7dbl_4, self.branch7x7dbl_5):
+            d = m(d)
+        return torch.cat([self.branch1x1(x), b7, d, self.branch_pool(_avg3(x))], 1)
+
+
+class _BlockE(tvi.InceptionE):
+    def __init__(self, in_channels, pool):
+        super().__init__(in_channels)
+        self.pool = pool
+
+    def forward(self, x):
+        b3 = self.branch3x3_1(x)
+        b3 = torch.cat([self.branch3x3_2a(b3), self.branch3x3_2b(b3)], 1)
+        d = self.branch3x3dbl_2(self.branch3x3dbl_1(x))
+        d = torch.cat([self.branch3x3dbl_3a(d), self.branch3x3dbl_3b(d)], 1)
+        return torch.cat([self.branch1x1(x), b3, d, self.branch_pool(self.pool(x))], 1)
+
+
+def weights_path():
+    """Where the FID weights live: the torch hub checkpoint directory, as ``load_state_dict_from_url`` would keep them."""
+    return os.path.join(torch.hub.get_dir(), "checkpoints", FID_WEIGHTS_URL.rsplit("/", 1)[-1])
+
+
+def fid_inception_v3():
+    """torchvision's Inception3 patched into the FID network, with the FID weights loaded ``strict=True``.  The weights are
+    fetched into the hub checkpoint directory only when they are not there yet."""
+    net = tvi.Inception3(num_classes=1008, aux_logits=False, init_weights=False)
+    net.Mixed_5b = _BlockA(192, pool_features=32)
+    net.Mixed_5c = _BlockA(256, pool_features=64)
+    net.Mixed_5d = _BlockA(288, pool_features=64)
+    for name, c7 in (("Mixed_6b", 128), ("Mixed_6c", 160), ("Mixed_6d", 160), ("Mixed_6e", 192)):
+        setattr(net, name, _BlockC(768, channels_7x7=c7))
+    net.Mixed_7b = _BlockE(1280, _avg3)
+    net.Mixed_7c = _BlockE(2048, _max3)
+    path = weights_path()
+    if not os.path.isfile(path):
+        os.makedirs(os.path.dirname(path), exist_ok=True)
+        torch.hub.download_url_to_file(FID_WEIGHTS_URL, path)
+    net.load_state_dict(torch.load(path, map_location="cpu"), strict=True)
+    return net
+
+
+class InceptionV3(nn.Module):
+    """Feature maps of the FID Inception (inception.py:20-169): block 0 ends at the first max pool (64 channels), block 1 at the
+    second (192), block 2 before the auxiliary classifier (768) and block 3 at the final average pool (2048).
+    ``forward(x)`` returns the requested blocks' outputs in ascending order.  ``x`` is expected in [0, 1] with
+    ``normalize_input`` and in [-1, 1] without; with ``resize_input`` it is first resized bilinearly to 299 x 299."""
+
+    DEFAULT_BLOCK_INDEX = 3
+    BLOCK_INDEX_BY_DIM = {64: 0, 192: 1, 768: 2, 2048: 3}
+
+    def __init__(self, output_blocks=(DEFAULT_BLOCK_INDEX,), resize_input=True, normalize_input=False, requires_grad=False,
+                 use_fid_inception=True):
+        super().__init__()
+        if not use_fid_inception:
+            raise ValueError("only the FID Inception (use_fid_inception=True) is provided")
+        self.resize_input = resize_input
+        self.normalize_input = normalize_input
+        self.output_blocks = sorted(output_blocks)
+        self.last_needed_block = max(output_blocks)
+        assert self.last_needed_block <= 3, "Last possible output block index is 3"
+        net = fid_inception_v3()
+        stages = [
+            [net.Conv2d_1a_3x3, net.Conv2d_2a_3x3, net.Conv2d_2b_3x3, nn.MaxPool2d(kernel_size=3, stride=2)],
+            [net.Conv2d_3b_1x1, net.Conv2d_4a_3x3, nn.MaxPool2d(kernel_size=3, stride=2)],
+            [net.Mixed_5b, net.Mixed_5c, net.Mixed_5d, net.Mixed_6a, net.Mixed_6b, net.Mixed_6c, net.Mixed_6d, net.Mixed_6e],
+            [net.Mixed_7a, net.Mixed_7b, net.Mixed_7c, nn.AdaptiveAvgPool2d(output_size=(1, 1))],
+        ]
+        self.blocks = nn.ModuleList(nn.Sequential(*s) for s in stages[:self.last_needed_block + 1])
+        self.requires_grad_(requires_grad)
+
+    def forward(self, inp):
+        x = inp
+        if self.resize_input:
+            x = F.interpolate(x, size=(299, 299), mode="bilinear", align_corners=False)
+        if self.normalize_input:
+            x = 2 * x - 1
+        out = []
+        for i, block in enumerate(self.blocks):
+            x = block(x)
+            if i in self.output_blocks:
+                out.append(x)
+        return out
+
+
+def seeded_state_dict(seed=0):
+    """A deterministic stand-in for the FID weights, for tests and benchmarks that must not reach the network: every
+    floating entry of the FID network's state dict drawn from ``torch.Generator().manual_seed(seed)`` in key order --
+    convolution / fc weights N(0, 2 / fan_in), BatchNorm weights 1 + 0.1 N(0, 1), biases and running means 0.1 N(0, 1),
+    running variances U(0.5, 1.5) (positive) -- and ``num_batches_tracked`` = 0."""
+    net = tvi.Inception3(num_classes=1008, aux_logits=False, init_weights=False)
+    g = torch.Generator().manual_seed(seed)
+    out = {}
+    for k, v in net.state_dict().items():
+        if k.endswith("num_batches_tracked"):
+            out[k] = torch.zeros_like(v)
+        elif k.endswith("running_var"):
+            out[k] = torch.rand(v.shape, generator=g) + 0.5
+        elif k.endswith("bn.weight"):
+            out[k] = 1 + 0.1 * torch.randn(v.shape, generator=g)
+        elif k.endswith("weight"):
+            out[k] = torch.randn(v.shape, generator=g) * (2.0 / v[0].numel()) ** 0.5
+        else:                                   # biases, running means
+            out[k] = 0.1 * torch.randn(v.shape, generator=g)
+    return out

@@ -1,5 +1,6 @@
-"""Improved precision and recall (Kynkäänniemi et al., 2019) of ``ddpm_torch/metrics/precision_recall.py``, with its k-NN
-half on the engine.
+"""The evaluation metrics of ``ddpm_torch/metrics``: improved precision and recall (Kynkäänniemi et al., 2019) of
+``precision_recall.py`` with its k-NN half on the engine, and FID (``fid_score.py``, ``__init__.py``'s ``Evaluator``) with its
+statistics and Fréchet distance on the engine (see the FID section below).
 
 Public names, signatures and defaults are the reference's: ``Manifold``, ``ManifoldBuilder``, ``calc_pr``,
 ``compute_distance``, ``to_uint8`` and ``VGGFeatureExtractor``.
@@ -21,6 +22,7 @@ from collections import namedtuple
 import numpy as np
 import torch
 import torch.nn as nn
+import torch.nn.functional as F
 from torch.utils.data import DataLoader, Subset
 
 from . import _lib
@@ -272,3 +274,307 @@ def calc_pr(manifold_1: Manifold, manifold_2: Manifold, row_batch_size: int, col
         return torch.cat(pred).to(torch.float32).mean()
 
     return coverage(f1, f2, k2), coverage(f2, f1, k1)
+
+
+# ================================================================================================ FID (fid_score.py)
+# * CUDA ``device``: InceptionStatistics keeps fp64 shift / sum / co-moment state on the device and folds each batch of features in
+#   with ``ddpm_fid_stats_update`` (a DMMA GEMM, csrc/fid.cuh) on that device's current stream; calc_fd runs ``ddpm_fid_distance``
+#   (two one-sided Jacobi eigen-solves and two DMMA GEMMs), with no scipy.linalg.sqrtm.  Only the final statistics and the distance
+#   come back to the host.
+# * CPU ``device``: the reference's numpy formulas.
+# Three upstream bugs are fixed, each next to its code: sqrtm's removed ``disp`` keyword (calculate_frechet_distance), numpy
+# features handed to adaptive_avg_pool2d for activation_dim != 2048 (InceptionStatistics.forward), and the empty last batch of
+# Evaluator.eval when the batch size divides the total.
+
+from .inception import InceptionV3, FID_WEIGHTS_URL  # noqa: E402
+
+IMAGE_RES = 299
+FID_STATUS = {1: "a non-finite input", 2: "sigma1 (mean1's covariance) is not positive semi-definite",
+              3: "sigma2 (mean2's covariance) is not positive semi-definite",
+              4: "the eigen-solve of sigma1 did not converge", 5: "the eigen-solve of L^T sigma2 L did not converge"}
+FID_NEG_TOL = 1e-6            # csrc/fid.cuh: lam_min < -1e-6 lam_max is not rounding
+
+
+class InceptionStatistics(nn.Module):
+    """fid_score.py:79-147: mean and covariance of the Inception features of every batch passed to ``forward``.
+
+    On a CUDA ``device`` (or the first device of a list, where Inception runs under ``DataParallel`` as upstream) the statistics
+    live in the native fp64 state on that device; on the CPU they follow the reference's per-batch ``np.cov`` and merge.
+    ``get_statistics()`` returns numpy fp64 ``(mean, cov)`` with cov divided by ``count - 1``; ``running_mean`` /
+    ``running_var`` are the population values (read-only)."""
+
+    def __init__(self, input_transform=lambda x: x, activation_dim=2048, device=torch.device("cpu")):
+        super().__init__()
+        self.input_transform = input_transform
+        self.activation_dim = activation_dim
+        self.device = device
+        self.model = self.load_model()
+        self._dev = _cuda_device(_op_device(device))
+        self.count = 0
+        if self._dev is not None:
+            nbytes = _lib.lib().ddpm_fid_stats_bytes(activation_dim)
+            _lib.check(0 if nbytes > 0 else int(nbytes), "fid_stats_bytes")
+            self._state = torch.zeros(nbytes, dtype=torch.uint8, device=self._dev)
+        else:
+            self._mean = np.zeros((activation_dim,), dtype=np.float64)
+            self._var = np.zeros((activation_dim, activation_dim), dtype=np.float64)
+
+    def load_model(self):
+        model = InceptionV3([InceptionV3.BLOCK_INDEX_BY_DIM[self.activation_dim]])
+        model.eval()
+        model.requires_grad_(False)
+        extractor = _FirstOutput(model)
+        if isinstance(self.device, (list, tuple)):
+            model.to(self.device[0])
+            return nn.DataParallel(extractor, device_ids=list(self.device))
+        return extractor.to(self.device)
+
+    def forward(self, x):
+        x = self.input_transform(x)
+        with torch.inference_mode():
+            act = self.model(x)
+            # Upstream pools after .cpu().numpy(), and adaptive_avg_pool2d refuses a numpy array: activation_dim 64 / 192 / 768
+            # raised TypeError.  Pooled here, on the features' own device, before they leave it.
+            if act.shape[2] != 1 or act.shape[3] != 1:
+                act = F.adaptive_avg_pool2d(act, (1, 1))
+            act = act.flatten(1)
+        n = act.shape[0]
+        if n == 0:
+            return
+        if self._dev is not None:
+            feats = act.to(device=self._dev, dtype=torch.float32).contiguous()
+            with torch.cuda.device(self._dev):
+                _lib.check(_lib.lib().ddpm_fid_stats_update(self._state.data_ptr(), self.activation_dim, feats.data_ptr(), n,
+                                                            feats.stride(0), _lib.stream_ptr(self._dev)), "InceptionStatistics")
+            self.count += n
+            return
+        act = act.cpu().numpy()
+        mean = np.mean(act, axis=0, dtype=np.float64)
+        var = np.cov(act, rowvar=False, ddof=0, dtype=np.float64)
+        alpha = n / (self.count + n)
+        if self.count == 0:
+            self._mean += mean
+            self._var += var
+        else:
+            diff = mean - self._mean
+            self._mean += alpha * diff
+            self._var += alpha * (var - self._var)
+            self._var += alpha * (1 - alpha) * np.outer(diff, diff)
+        self.count += n
+
+    def _native_stats(self, ddof):
+        D = self.activation_dim
+        with torch.cuda.device(self._dev):
+            mean = torch.empty(D, dtype=torch.float64, device=self._dev)
+            cov = torch.empty(D, D, dtype=torch.float64, device=self._dev)
+            _lib.check(_lib.lib().ddpm_fid_stats_finalize(self._state.data_ptr(), D, self.count, ddof, mean.data_ptr(),
+                                                          cov.data_ptr(), _lib.stream_ptr(self._dev)), "InceptionStatistics")
+            return mean.cpu().numpy(), cov.cpu().numpy()
+
+    @property
+    def running_mean(self):
+        if self._dev is None:
+            return _readonly(self._mean)
+        if self.count == 0:
+            return _readonly(np.zeros(self.activation_dim))
+        return _readonly(self._native_stats(0)[0])
+
+    @property
+    def running_var(self):
+        if self._dev is None:
+            return _readonly(self._var)
+        if self.count == 0:
+            return _readonly(np.zeros((self.activation_dim, self.activation_dim)))
+        return _readonly(self._native_stats(0)[1])
+
+    def get_statistics(self):
+        assert self.count > 1, "Count must be greater than 1!"
+        if self._dev is not None:
+            return self._native_stats(1)
+        return self._mean.copy(), self._var.copy() * self.count / (self.count - 1)
+
+    def reset(self):
+        if self._dev is not None:
+            self._state.zero_()
+        else:
+            self._mean.fill(0)
+            self._var.fill(0)
+        self.count = 0
+
+
+class _FirstOutput(nn.Module):
+    def __init__(self, module):
+        super().__init__()
+        self._module = module
+
+    def forward(self, x):
+        return self._module(x)[0]
+
+
+def _readonly(a):
+    a = a.view()
+    a.flags.writeable = False
+    return a
+
+
+# fid_score.py:150-158
+PRE_COMPUTED_LIST = {
+    "celeba": "https://github.com/tqch/VAEGAN/releases/download/precomputed_statistics_celeba/fid_stats_celeba_148x148.npz",
+    "lsun_bedroom": "http://bioinf.jku.at/research/ttur/ttur_stats/fid_stats_lsun_train.npz",
+    "cifar10": "http://bioinf.jku.at/research/ttur/ttur_stats/fid_stats_cifar10_train.npz",
+    "svhn": "http://bioinf.jku.at/research/ttur/ttur_stats/fid_stats_svhn_train.npz",
+    "imagenet_train": "http://bioinf.jku.at/research/ttur/ttur_stats/fid_stats_imagenet_train.npz",
+    "imagenet_valid": "http://bioinf.jku.at/research/ttur/ttur_stats/fid_stats_imagenet_valid.npz",
+}
+
+
+def get_precomputed(dataset, download_dir="precomputed"):
+    """fid_score.py:161-183: ``(mu, sigma)`` of the dataset's precomputed statistics, read from ``download_dir`` and fetched
+    into it only when the file is absent (``download_dir=None``: fetched into memory)."""
+    url = PRE_COMPUTED_LIST.get(dataset, f"fid_stats_{dataset}.npz")
+    name = os.path.basename(url)
+    if download_dir is None:
+        import io
+        import requests
+        src = io.BytesIO(requests.get(url).content)
+    else:
+        src = os.path.join(download_dir, name)
+        if not os.path.exists(src):
+            import requests
+            os.makedirs(download_dir, exist_ok=True)
+            r = requests.get(url, timeout=120)
+            assert r.status_code == 200
+            with open(src, "wb") as f:
+                f.write(r.content)
+    data = np.load(src)
+    return data["mu"], data["sigma"]
+
+
+def _sqrtm(a):
+    """scipy.linalg.sqrtm(a) as a matrix.  Upstream calls ``sqrtm(..., disp=False)``, a keyword SciPy has removed (1.18 raises
+    TypeError), so calc_fd did not run at all; with that keyword gone the matrix is the whole return value."""
+    from scipy import linalg
+    try:
+        return linalg.sqrtm(a, disp=False)[0]
+    except TypeError:
+        return linalg.sqrtm(a)
+
+
+def calculate_frechet_distance(mu1, sigma1, mu2, sigma2, eps=1e-6):
+    """fid_score.py:269-323 on the CPU: ||mu1 - mu2||^2 + tr(sigma1 + sigma2 - 2 sqrtm(sigma1 sigma2)), with ``eps`` added to both
+    diagonals when the product's square root is not finite, and a ValueError when it has a significant imaginary part."""
+    mu1, mu2 = np.atleast_1d(mu1), np.atleast_1d(mu2)
+    sigma1, sigma2 = np.atleast_2d(sigma1), np.atleast_2d(sigma2)
+    assert mu1.shape == mu2.shape, "Training and test mean vectors have different lengths"
+    assert sigma1.shape == sigma2.shape, "Training and test covariances have different dimensions"
+    diff = mu1 - mu2
+    covmean = _sqrtm(sigma1.dot(sigma2))
+    if not np.isfinite(covmean).all():
+        print(f"fid calculation produces singular product; adding {eps} to diagonal of cov estimates")
+        offset = np.eye(sigma1.shape[0]) * eps
+        covmean = _sqrtm((sigma1 + offset).dot(sigma2 + offset))
+    if np.iscomplexobj(covmean):
+        if not np.allclose(np.diagonal(covmean).imag, 0, atol=1e-3):
+            raise ValueError("Imaginary component {}".format(np.max(np.abs(covmean.imag))))
+        covmean = covmean.real
+    return diff.dot(diff) + np.trace(sigma1) + np.trace(sigma2) - 2 * np.trace(covmean)
+
+
+def _fd_device(args, device):
+    if device is not None:
+        return _cuda_device(_op_device(device))
+    for a in args:
+        if isinstance(a, torch.Tensor) and a.is_cuda:
+            return a.device
+    return torch.device("cuda", torch.cuda.current_device()) if torch.cuda.is_available() else None
+
+
+def frechet_distance_native(mean1, var1, mean2, var2, device):
+    """``ddpm_fid_distance`` on ``device``'s current stream.  Returns ``(fd, info)``: ``info`` holds the status, the sweep counts of
+    both eigen-solves, the most negative eigenvalue of sigma1 and of M = L^T sigma2 L relative to their largest, and
+    tr sqrt(sigma1 sigma2).  Raises ValueError for non-finite or non-PSD input, RuntimeError when an eigen-solve did not converge."""
+    dev = _cuda_device(device)
+    L = _lib.lib()
+    with torch.cuda.device(dev):
+        t = [torch.as_tensor(np.asarray(a) if not isinstance(a, torch.Tensor) else a).to(device=dev, dtype=torch.float64)
+             for a in (mean1, var1, mean2, var2)]
+        mu1, s1, mu2, s2 = (t[0].reshape(-1).contiguous(), t[1].reshape(t[1].shape[0] if t[1].dim() else 1, -1).contiguous(),
+                            t[2].reshape(-1).contiguous(), t[3].reshape(t[3].shape[0] if t[3].dim() else 1, -1).contiguous())
+        assert mu1.shape == mu2.shape, "Training and test mean vectors have different lengths"
+        assert s1.shape == s2.shape, "Training and test covariances have different dimensions"
+        D = mu1.shape[0]
+        if s1.shape != (D, D):
+            raise ValueError(f"covariances must be {D} x {D} to match the means, got {tuple(s1.shape)}")
+        nbytes = L.ddpm_fid_distance_scratch_bytes(D)
+        if nbytes < 0:
+            _lib.check(int(nbytes), "fid_distance_scratch_bytes")
+        scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        out = torch.full((8,), float("nan"), dtype=torch.float64, device=dev)
+        _lib.check(L.ddpm_fid_distance(mu1.data_ptr(), s1.data_ptr(), mu2.data_ptr(), s2.data_ptr(), D, out.data_ptr(),
+                                       scratch.data_ptr(), nbytes, _lib.stream_ptr(dev)), "calc_fd")
+        o = out.cpu().numpy()
+    status = int(o[1])
+    info = {"status": status, "sweeps": (int(o[2]), int(o[3])), "min_ratio": (float(o[4]), float(o[5])), "tr_sqrt": float(o[6])}
+    if status in (1, 2, 3):
+        ratio = f" (lam_min / lam_max = {o[3 + status]:.3e}, below -{FID_NEG_TOL:g})" if status > 1 else ""
+        raise ValueError(f"calc_fd: {FID_STATUS[status]}{ratio}")
+    if status:
+        raise RuntimeError(f"calc_fd: {FID_STATUS[status]}")
+    return np.float64(o[0]), info
+
+
+def calc_fd(mean1, var1, mean2, var2, eps=1e-6, device=None):
+    """fid_score.py:186-187.  On the device of a CUDA tensor argument, on ``device``, or else on the current CUDA device when one
+    is present: the native eigenvalue route (``frechet_distance_native``).  ``eps`` is accepted for the reference's signature and
+    never needed there: the route takes no square root of a possibly singular product, so there is no diagonal offset to
+    retry with.  Non-PSD input raises ValueError, the counterpart of upstream's "Imaginary component" error.  Otherwise (a CPU
+    ``device``, or no CUDA device): the reference formula, ``calculate_frechet_distance``.  Returns a numpy float64."""
+    dev = _fd_device((mean1, var1, mean2, var2), device)
+    if dev is None:
+        args = [a.detach().cpu().numpy() if isinstance(a, torch.Tensor) else a for a in (mean1, var1, mean2, var2)]
+        return calculate_frechet_distance(*args, eps)
+    return frechet_distance_native(mean1, var1, mean2, var2, dev)[0]
+
+
+class Evaluator:
+    """metrics/__init__.py:18-53: FID of ``eval_total_size`` samples drawn ``eval_batch_size`` at a time, against the dataset's
+    precomputed statistics."""
+
+    def __init__(self, dataset, diffusion=None, eval_batch_size=256, eval_total_size=50000, device=torch.device("cpu")):
+        self.diffusion = diffusion
+        self.istats = InceptionStatistics(device=device)
+        self.eval_batch_size = eval_batch_size
+        self.eval_total_size = eval_total_size
+        self.device = device
+        self.target_mean, self.target_var = get_precomputed(dataset)
+
+    def eval(self, sample_fn, is_leader=True):
+        try:
+            from tqdm import trange
+        except ImportError:
+            def trange(n, **kw):
+                return range(n)
+        if is_leader:
+            self.istats.reset()
+        fid = None
+        num_batches = math.ceil(self.eval_total_size / self.eval_batch_size)
+        with trange(num_batches, desc="Evaluating FID", disable=not is_leader) as t:
+            for i in t:
+                batch_size = self.eval_batch_size
+                if i == num_batches - 1:
+                    # Upstream takes eval_total_size % eval_batch_size, which is 0 when the batch size divides the total: the
+                    # empty batch's NaN mean then turned the running statistics, and the FID, into NaN.
+                    batch_size = self.eval_total_size - self.eval_batch_size * (num_batches - 1)
+                x = sample_fn(sample_size=batch_size, diffusion=self.diffusion)
+                if is_leader:
+                    op = _op_device(self.device)
+                    self.istats(x.to(op))
+                    if i == num_batches - 1:
+                        gen_mean, gen_var = self.istats.get_statistics()
+                        fid = calc_fd(gen_mean, gen_var, self.target_mean, self.target_var, device=op)
+                        t.set_postfix({"fid": fid})
+        return {"fid": fid}
+
+
+__all__ = ["Manifold", "ManifoldBuilder", "calc_pr", "compute_distance", "to_uint8", "VGGFeatureExtractor",
+           "InceptionV3", "InceptionStatistics", "get_precomputed", "calc_fd", "calculate_frechet_distance", "Evaluator"]

@@ -201,6 +201,28 @@ int ddpm_knn_cover(const void* probes, int n_probes, long long ld_p, const void*
                    const void* radii, uint8_t* covered, void* scratch, long long bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Fréchet Inception Distance (ddpm_torch/metrics/fid_score.py), fp64 throughout, on the fp64 tensor cores (DMMA) where it is a
+ * contraction (fid.cuh).  D in 1..4096.  No allocation, no synchronisation; results are bit-identical from call to call, and every
+ * argument error is refused before any device work.
+ * ddpm_fid_stats_update   (InceptionStatistics.forward, :116-135): folds n rows of fp32 features feats[n][ld] (device, 4-byte
+ *                         aligned, ld >= D) into the state: state bytes = ddpm_fid_stats_bytes(D), 16-byte aligned, zero-filled by the
+ *                         caller before the first update (and to reset).  The row count stays with the caller; n = 0 is a no-op.
+ * ddpm_fid_stats_finalize (:137-142): mean f64[D] and cov f64[D][D] (full, symmetric) of the n rows folded in so far, cov divided by
+ *                         n - ddof (ddof 1: get_statistics; ddof 0: the population running values).  Needs n > ddof.
+ * ddpm_fid_distance       (calc_fd / calculate_frechet_distance, :186-187, :269-323): mu f64[D], sigma f64[D][D] (device);
+ *                         out f64[8] (device) <- {fd, status, sweeps(sigma1), sweeps(M), lam_min/lam_max(sigma1),
+ *                         nu_min/nu_max(M), tr sqrt(sigma1 sigma2), 0} with M = L^T sigma2 L, sigma1 = L L^T.  status: 0 ok,
+ *                         1 non-finite input, 2 sigma1 not PSD (lam_min < -1e-6 lam_max), 3 M not PSD (sigma2 not PSD),
+ *                         4 / 5 eigen-solve of sigma1 / M did not converge within 60 sweeps; fd is NaN unless status is 0.
+ *                         scratch: ddpm_fid_distance_scratch_bytes(D) bytes, 16-byte aligned, no initialisation needed. */
+long long ddpm_fid_stats_bytes(int D);
+int ddpm_fid_stats_update(void* state, int D, const float* feats, long long n, long long ld, void* stream);
+int ddpm_fid_stats_finalize(const void* state, int D, long long n, int ddof, double* mean_out, double* cov_out, void* stream);
+long long ddpm_fid_distance_scratch_bytes(int D);
+int ddpm_fid_distance(const double* mu1, const double* sigma1, const double* mu2, const double* sigma2, int D, double* out,
+                      void* scratch, long long bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Low-level operators: GroupNorm(32, C, eps=1e-6) [+ SiLU] [+ dropout] (unet.py:18-20,83-84) and the bias column sums, with the
  * launch geometry the UNet engine's plans use (used by the parity tests of the engine itself).
  * Input = channel concat of two NHWC bf16 sources x0 [B][HW][C0] and x1 [B][HW][C1] (C1 = 0: one source).  C0 and C1 are
