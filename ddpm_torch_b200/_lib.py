@@ -193,6 +193,13 @@ def lib():
             "ddpm_fid_stats_finalize": ([vp, i32, i64, i32, vp, vp, vp], i32),
             "ddpm_fid_distance_scratch_bytes": ([i32], i64),
             "ddpm_fid_distance": ([vp, vp, vp, vp, i32, vp, vp, i64, vp], i32),
+            "ddpm_toy_num_params": ([vp], i64),
+            "ddpm_toy_workspace_bytes": ([vp, i64, i32], i64),
+            "ddpm_toy_forward": ([vp, vp, vp, vp, i64, vp, i32, vp, i64, vp], i32),
+            "ddpm_toy_train_forward": ([vp, vp, vp, vp, vp, vp, vp, i64, vp, vp, i64, vp], i32),
+            "ddpm_toy_backward": ([vp, vp, vp, vp, i64, vp, vp, vp, i64, vp], i32),
+            "ddpm_toy_train_backward": ([vp, vp, vp, vp, vp, i64, vp, vp, i64, vp], i32),
+            "ddpm_toy_sample": ([vp, vp, vp, i64, i32, vp, vp, vp, i64, vp], i32),
         }
         for name, (args, res) in sig.items():
             fn = getattr(L, name)
@@ -214,7 +221,8 @@ EXPORTS = ["ddpm_last_error", "ddpm_runtime_check", "ddpm_device_error_flag", "d
            "ddpm_unet_temb_layout", "ddpm_unet_temb_forward", "ddpm_unet_temb_backward",
            "ddpm_knn_scratch_bytes", "ddpm_knn_kth", "ddpm_knn_cover",
            "ddpm_fid_stats_bytes", "ddpm_fid_stats_update", "ddpm_fid_stats_finalize", "ddpm_fid_distance_scratch_bytes",
-           "ddpm_fid_distance"]
+           "ddpm_fid_distance", "ddpm_toy_num_params", "ddpm_toy_workspace_bytes", "ddpm_toy_forward", "ddpm_toy_train_forward",
+           "ddpm_toy_backward", "ddpm_toy_train_backward", "ddpm_toy_sample"]
 
 
 def check(rc, what=""):

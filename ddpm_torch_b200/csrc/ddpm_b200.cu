@@ -8,6 +8,7 @@
 #include "optim.cuh"
 #include "knn.cuh"
 #include "fid.cuh"
+#include "toy_mlp.cuh"
 
 using namespace ddpm;
 
@@ -943,6 +944,122 @@ int ddpm_unet_temb_backward(ddpm_unet* h, const float* dtp, float* d_st, float* 
     if (d_st) DDPM_CUDA_OK(cudaMemcpyAsync(d_st, e.temb.d_st, (size_t)e.B * e.temb.E * 4, cudaMemcpyDefault, st));
     if (d_s0) DDPM_CUDA_OK(cudaMemcpyAsync(d_s0, e.temb.d_s0, (size_t)e.B * e.temb.E * 4, cudaMemcpyDefault, st));
     return 0;
+}
+
+// ------------------------------------------------------------------------------------------------ 2-D toy denoiser (toy_mlp.cuh)
+static int toy_check(const char* fn, const ddpm_toy_cfg* c, long long B) {
+    if (!c) return fail(-47, "%s: null config", fn);
+    if (c->mid_features != 64 && c->mid_features != 128)
+        return fail(-47, "%s: mid_features = %d unsupported (native: 64 or 128, the weights stay resident in shared memory)", fn, c->mid_features);
+    if (c->in_features < 1 || c->in_features > 4) return fail(-47, "%s: in_features = %d unsupported (native: 1..4)", fn, c->in_features);
+    if (c->num_layers < 1) return fail(-47, "%s: num_temporal_layers must be >= 1 (got %d)", fn, c->num_layers);
+    if (B < 1 || B > (1LL << 24)) return fail(-47, "%s: rows must be in 1..2^24 (got %lld)", fn, B);
+    return 0;
+}
+static int toy_check_params(const char* fn, const ddpm_toy_params* p) {
+    if (!p) return fail(-47, "%s: null parameter table", fn);
+    const float* const* a = &p->in_fc_weight;
+    for (int i = 0; i < 15; ++i)
+        if (!a[i]) return fail(-47, "%s: parameter %d is null", fn, i);
+    if (misaligned16(p->fc1_weight) || misaligned16(p->fc2_weight) || misaligned16(p->enc_weight) || misaligned16(p->t_proj_weight))
+        return fail(-47, "%s: the [M][M] weights must be 16-byte aligned", fn);
+    return 0;
+}
+static int toy_check_ws(const char* fn, const ddpm_toy_cfg* c, long long rows, int training, const void* ws, long long bytes) {
+    const size_t need = toy_ws_layout(c->mid_features, c->in_features, c->num_layers, rows, training).total;
+    if (!ws || (reinterpret_cast<uintptr_t>(ws) & 255) || bytes < (long long)need)
+        return fail(-47, "%s: needs a 256-byte aligned workspace of ddpm_toy_workspace_bytes = %zu bytes (got %lld)", fn, need, bytes);
+    return 0;
+}
+static ToyArgs toy_args(const ddpm_toy_cfg* c, const ddpm_toy_params* p, long long B, void* ws, int training) {
+    ToyArgs a; memset(&a, 0, sizeof a);
+    a.w = *p; a.M = c->mid_features; a.D = c->in_features; a.L = c->num_layers; a.B = (int)B;
+    const ToyWs l = toy_ws_layout(a.M, a.D, a.L, B, training);
+    uint8_t* b = static_cast<uint8_t*>(ws);
+    a.E = reinterpret_cast<float*>(b + l.E);
+    if (training) {
+        a.h_sv = reinterpret_cast<float*>(b + l.h); a.u_sv = reinterpret_cast<float*>(b + l.u);
+        a.x_sv = reinterpret_cast<float*>(b + l.x); a.out_sv = reinterpret_cast<float*>(b + l.out);
+        a.dE = reinterpret_cast<float*>(b + l.dE); a.part = reinterpret_cast<float*>(b + l.part);
+    }
+    return a;
+}
+static int toy_done(const char* fn, cudaError_t e) { return e == cudaSuccess ? 0 : fail(-20, "%s: launch failed: %s", fn, cudaGetErrorString(e)); }
+
+long long ddpm_toy_num_params(const ddpm_toy_cfg* cfg) {
+    if (int rc = toy_check("ddpm_toy_num_params", cfg, 1)) return rc;
+    return ToyLayout(cfg->mid_features, cfg->in_features, cfg->num_layers).P;
+}
+
+long long ddpm_toy_workspace_bytes(const ddpm_toy_cfg* cfg, long long rows, int training) {
+    if (int rc = toy_check("ddpm_toy_workspace_bytes", cfg, rows)) return rc;
+    return (long long)toy_ws_layout(cfg->mid_features, cfg->in_features, cfg->num_layers, rows, training ? 1 : 0).total;
+}
+
+int ddpm_toy_forward(const ddpm_toy_cfg* cfg, const ddpm_toy_params* p, const float* x, const long long* t, long long B, float* out,
+                     int training, void* ws, long long ws_bytes, void* stream) {
+    const char* fn = "ddpm_toy_forward";
+    if (int rc = toy_check(fn, cfg, B)) return rc;
+    if (int rc = toy_check_params(fn, p)) return rc;
+    if (!x || !t || !out) return fail(-47, "%s: null x, t or out", fn);
+    if (int rc = toy_check_ws(fn, cfg, B, training ? 1 : 0, ws, ws_bytes)) return rc;
+    ToyArgs a = toy_args(cfg, p, B, ws, training ? 1 : 0);
+    a.x = x; a.t = t; a.out = out;
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    return toy_done(fn, a.M == 64 ? toy_forward_launch<64>(a, st) : toy_forward_launch<128>(a, st));
+}
+
+int ddpm_toy_train_forward(const ddpm_toy_cfg* cfg, const ddpm_toy_params* p, const float* x0, const long long* t, const float* noise,
+                           const float* sqrt_ab, const float* sqrt_1mab, long long B, float* losses, void* ws, long long ws_bytes,
+                           void* stream) {
+    const char* fn = "ddpm_toy_train_forward";
+    if (int rc = toy_check(fn, cfg, B)) return rc;
+    if (int rc = toy_check_params(fn, p)) return rc;
+    if (!x0 || !t || !noise || !sqrt_ab || !sqrt_1mab || !losses) return fail(-47, "%s: null input or output", fn);
+    if (int rc = toy_check_ws(fn, cfg, B, 1, ws, ws_bytes)) return rc;
+    ToyArgs a = toy_args(cfg, p, B, ws, 1);
+    a.x0 = x0; a.t = t; a.noise = noise; a.sa = sqrt_ab; a.s1a = sqrt_1mab; a.loss = losses;
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    return toy_done(fn, a.M == 64 ? toy_forward_launch<64>(a, st) : toy_forward_launch<128>(a, st));
+}
+
+static int toy_backward_common(const char* fn, const ddpm_toy_cfg* cfg, const ddpm_toy_params* p, const long long* t, long long B,
+                               const float* d_out, const float* noise, const float* g, float* dx, float* grad, void* ws,
+                               long long ws_bytes, void* stream) {
+    if (int rc = toy_check(fn, cfg, B)) return rc;
+    if (int rc = toy_check_params(fn, p)) return rc;
+    if (!t || !grad || (!d_out && !(noise && g))) return fail(-47, "%s: null t, seed gradient or grad", fn);
+    if (int rc = toy_check_ws(fn, cfg, B, 1, ws, ws_bytes)) return rc;
+    ToyArgs a = toy_args(cfg, p, B, ws, 1);
+    a.t = t; a.d_out = d_out; a.noise = noise; a.g = g; a.dx = dx;
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    return toy_done(fn, a.M == 64 ? toy_backward_launch<64>(a, grad, st) : toy_backward_launch<128>(a, grad, st));
+}
+
+int ddpm_toy_backward(const ddpm_toy_cfg* cfg, const ddpm_toy_params* p, const long long* t, const float* d_out, long long B,
+                      float* dx, float* grad, void* ws, long long ws_bytes, void* stream) {
+    if (!d_out) return fail(-47, "ddpm_toy_backward: null d_out");
+    return toy_backward_common("ddpm_toy_backward", cfg, p, t, B, d_out, nullptr, nullptr, dx, grad, ws, ws_bytes, stream);
+}
+
+int ddpm_toy_train_backward(const ddpm_toy_cfg* cfg, const ddpm_toy_params* p, const long long* t, const float* noise, const float* g,
+                            long long B, float* grad, void* ws, long long ws_bytes, void* stream) {
+    if (!noise || !g) return fail(-47, "ddpm_toy_train_backward: null noise or g");
+    return toy_backward_common("ddpm_toy_train_backward", cfg, p, t, B, nullptr, noise, g, nullptr, grad, ws, ws_bytes, stream);
+}
+
+int ddpm_toy_sample(const ddpm_toy_cfg* cfg, const ddpm_toy_params* p, float* x, long long B, int S, const float* coef,
+                    const float* z, void* ws, long long ws_bytes, void* stream) {
+    const char* fn = "ddpm_toy_sample";
+    if (int rc = toy_check(fn, cfg, B)) return rc;
+    if (int rc = toy_check_params(fn, p)) return rc;
+    if (S < 1 || S > 100000) return fail(-47, "%s: S must be in 1..100000 (got %d)", fn, S);
+    if (!x || !coef || !z) return fail(-47, "%s: null x, coef or z", fn);
+    if (int rc = toy_check_ws(fn, cfg, S, 0, ws, ws_bytes)) return rc;
+    ToyArgs a = toy_args(cfg, p, B, ws, 0);
+    a.x = x; a.coef = coef; a.z = z; a.S = S;
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    return toy_done(fn, a.M == 64 ? toy_sample_launch<64>(a, st) : toy_sample_launch<128>(a, st));
 }
 
 }  // extern "C"

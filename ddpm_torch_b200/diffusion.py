@@ -11,7 +11,8 @@ the configuration is the one every reference config uses (eps-prediction, fixed 
 * ``calc_all_bpd`` -> the engine's bits/dim step (q_sample, UNet forward and the variational-bound terms of
   diffusion.py:203-215 in one launch sequence, replayed from a CUDA graph once per timestep).
 
-Any other ``denoise_fn`` (toy MLPs, wrappers) takes the generic formulas below, written with plain torch ops.
+Any other ``denoise_fn`` (wrappers, other modules) takes the generic formulas below, written with plain torch ops; the toy models'
+native paths are in ``ddpm_torch_b200.toy``.
 """
 import ctypes as C
 

@@ -40,3 +40,11 @@ def discretized_gaussian_loglik(x, means, log_scale, precision=1. / 255, cutoff=
     hi = torch.where(x > cutoff[1], one, approx_std_normal_cdf(inv_std * (centered + precision)))
     lo = torch.where(x < cutoff[0], one * 0, approx_std_normal_cdf(inv_std * (centered - precision)))
     return torch.log((hi - lo - tol).clamp(min=0) + tol)
+
+
+def continuous_gaussian_loglik(x, mean, logvar):
+    """functions.py:78-83: element-wise log N(x; mean, exp(logvar)), the decoder term of the toy models' bound."""
+    x_centered = x - mean
+    inv_var = torch.exp(-logvar)
+    log_probs = x_centered.pow(2) * inv_var + math.log(2 * math.pi) + logvar
+    return log_probs.mul(0.5).neg()

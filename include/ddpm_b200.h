@@ -411,6 +411,42 @@ int ddpm_opt_step(float* params, const float* grads, float* exp_avg, float* exp_
  * layout PIL.Image.fromarray consumes (generate.py:112-114).  Bit-exact with the reference expression.  C in 1..4. */
 int ddpm_to_uint8_nhwc(const float* x, uint8_t* out, int B, int C, int H, int W, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * 2-D toy denoiser (ddpm_torch/toy/toy_model.py: Decoder(in_features, mid_features, num_temporal_layers)) on wgmma (toy_mlp.cuh).
+ * Stateless: every call takes the configuration and the current fp32 parameter pointers (device, in the reference's parameters()
+ * order; the four [M][M] weights 16-byte aligned), so updates by any optimiser or p.data.copy_ are seen without a repack.
+ * Supported: mid_features M in {64, 128}, in_features D in 1..4, num_layers L >= 1, B >= 1; anything else is refused before any
+ * launch.  No allocation, no synchronisation, graph-capturable; the caller's stream.
+ * ws: caller-owned device workspace of ddpm_toy_workspace_bytes(cfg, rows, training) bytes, 256-byte aligned.  A training forward
+ * fills it with what the matching backward reads, so it must be kept until that backward has run.
+ * ddpm_toy_forward        x f32 [B][D], t i64 [B] -> out f32 [B][D]; training != 0 saves the activations for ddpm_toy_backward
+ * ddpm_toy_train_forward  losses[b] = mean((noise - Decoder(q_sample(x0, t, noise), t))^2) with sqrt_ab / sqrt_1mab f32 [T] (always
+ *                         saves; workspace with training = 1)
+ * ddpm_toy_backward       d_out f32 [B][D] -> grad f32 [P] (flat, parameters() order, overwritten) and dx f32 [B][D] (optional)
+ * ddpm_toy_train_backward per-row loss gradient g f32 [B] (and the same noise) -> grad
+ * ddpm_toy_sample         the whole p_sample chain (toy/diffusion.py: no clip) in one launch after the step table: x f32 [B][D] in
+ *                         place, coef f32 [S][6] = {sqrt_recip_ab, sqrt_recip_m1_ab, coef1, coef2, sigma, t > 0}, z f32 [S][B][D]
+ *                         (z[k] at t = S-1-k); workspace ddpm_toy_workspace_bytes(cfg, S, 0)
+ * Gradients are summed in a fixed order (per-CTA partials, then one reduce): a training step is bit-reproducible. */
+typedef struct { int in_features, mid_features, num_layers; } ddpm_toy_cfg;
+typedef struct {
+    const float *in_fc_weight, *norm1_weight, *norm1_bias, *fc1_weight, *norm2_weight, *norm2_bias, *fc2_weight, *enc_weight,
+        *enc_bias, *out_norm_weight, *out_norm_bias, *out_fc_weight, *out_fc_bias, *t_proj_weight, *t_proj_bias;
+} ddpm_toy_params;
+long long ddpm_toy_num_params(const ddpm_toy_cfg* cfg);
+long long ddpm_toy_workspace_bytes(const ddpm_toy_cfg* cfg, long long rows, int training);
+int ddpm_toy_forward(const ddpm_toy_cfg* cfg, const ddpm_toy_params* p, const float* x, const long long* t, long long B, float* out,
+                     int training, void* ws, long long ws_bytes, void* stream);
+int ddpm_toy_train_forward(const ddpm_toy_cfg* cfg, const ddpm_toy_params* p, const float* x0, const long long* t, const float* noise,
+                           const float* sqrt_ab, const float* sqrt_1mab, long long B, float* losses, void* ws, long long ws_bytes,
+                           void* stream);
+int ddpm_toy_backward(const ddpm_toy_cfg* cfg, const ddpm_toy_params* p, const long long* t, const float* d_out, long long B,
+                      float* dx, float* grad, void* ws, long long ws_bytes, void* stream);
+int ddpm_toy_train_backward(const ddpm_toy_cfg* cfg, const ddpm_toy_params* p, const long long* t, const float* noise, const float* g,
+                            long long B, float* grad, void* ws, long long ws_bytes, void* stream);
+int ddpm_toy_sample(const ddpm_toy_cfg* cfg, const ddpm_toy_params* p, float* x, long long B, int S, const float* coef,
+                    const float* z, void* ws, long long ws_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
