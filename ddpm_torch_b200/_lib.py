@@ -157,6 +157,7 @@ def lib():
             "ddpm_unet_num_params": ([vp], i32),
             "ddpm_unet_param_info": ([vp, i32, C.POINTER(C.c_char_p), C.POINTER(i32), C.POINTER(i32 * 4), C.POINTER(i64)], i32),
             "ddpm_unet_flat_elems": ([vp], i64),
+            "ddpm_unet_graph_epoch": ([vp], i64),
             "ddpm_unet_workspace_bytes": ([vp, i32, i32, i32, i32], i64),
             "ddpm_unet_plan": ([vp, i32, i32, i32, i32, vp, vp, vp, i64], i32),
             "ddpm_unet_repack": ([vp, vp], i32),
@@ -213,7 +214,7 @@ EXPORTS = ["ddpm_last_error", "ddpm_runtime_check", "ddpm_device_error_flag", "d
            "ddpm_attention_fwd_run", "ddpm_attention_bwd_run", "ddpm_attn_scratch_bytes", "ddpm_conv_run", "ddpm_conv_scratch_bytes",
            "ddpm_gn_scratch_bytes", "ddpm_groupnorm_fwd_run", "ddpm_groupnorm_bwd_run", "ddpm_colsum_run",
            "ddpm_unet_create", "ddpm_unet_create_ex", "ddpm_unet_destroy", "ddpm_unet_num_params", "ddpm_unet_param_info",
-           "ddpm_unet_flat_elems", "ddpm_unet_workspace_bytes", "ddpm_unet_plan", "ddpm_unet_repack",
+           "ddpm_unet_flat_elems", "ddpm_unet_graph_epoch", "ddpm_unet_workspace_bytes", "ddpm_unet_plan", "ddpm_unet_repack",
            "ddpm_unet_forward", "ddpm_unet_backward", "ddpm_unet_backward_ex", "ddpm_unet_backward_launches", "ddpm_train_forward", "ddpm_train_backward",
            "ddpm_sampler_setup", "ddpm_sampler_reset", "ddpm_sampler_step", "ddpm_sampler_step_pred",
            "ddpm_bpd_setup", "ddpm_bpd_reset", "ddpm_bpd_step", "ddpm_unet_grad_chunks", "ddpm_unet_wait_grad_chunk", "ddpm_unet_plan_stats",

@@ -14,11 +14,12 @@ using namespace ddpm;
 
 struct ddpm_unet {
     UnetEngine e;
-    // sampler tables (device, owned by the handle; allocated by ddpm_sampler_setup, never per step)
-    long long* d_tmodel = nullptr; float* d_coef = nullptr; int S = 0;
+    // sampler tables (device, owned by the handle; allocated by ddpm_sampler_setup, never per step): t_model i64[S], coef f32[S][6]
+    void* d_samp = nullptr; int S = 0;
     // bits/dim tables (allocated by ddpm_bpd_setup; separate from the sampler's, whose addresses a captured sampler graph holds):
     // t_model i64[T] = 0..T-1, rows f32[T][kBpdRow], sqrt_ab f32[T], sqrt_1mab f32[T]
     void* d_bpd = nullptr; int bpd_T = 0;
+    long long graph_epoch = 0;     // moves whenever an address a captured launch holds may have moved (ddpm_unet_graph_epoch)
     const float* train_target = nullptr;
     bool temb_rows = false;        // the last forward of this plan was a per-row ddpm_unet_temb_forward (what its backward reads);
                                    // every other forward entry point clears it
@@ -561,8 +562,7 @@ int ddpm_unet_create_ex(const ddpm_unet_cfg* cfg, int resample_with_conv, ddpm_u
 }
 void ddpm_unet_destroy(ddpm_unet* h) {
     if (!h) return;
-    if (h->d_tmodel) cudaFree(h->d_tmodel);
-    if (h->d_coef) cudaFree(h->d_coef);
+    if (h->d_samp) cudaFree(h->d_samp);
     if (h->d_bpd) cudaFree(h->d_bpd);
     if (h->e.side_stream) { cudaStreamSynchronize(h->e.side_stream);   // a queued weight re-pack still writes into the caller's workspace
         cudaStreamDestroy(h->e.side_stream); cudaEventDestroy(h->e.ev_fork); cudaEventDestroy(h->e.ev_join); }
@@ -582,8 +582,13 @@ int ddpm_unet_param_info(const ddpm_unet* h, int i, const char** name, int* ndim
 }
 long long ddpm_unet_flat_elems(const ddpm_unet* h) { return h->e.flat_elems; }
 
+long long ddpm_unet_graph_epoch(const ddpm_unet* h) {
+    if (!h) return fail(-30, "ddpm_unet_graph_epoch: null handle");
+    return h->graph_epoch;
+}
 long long ddpm_unet_workspace_bytes(ddpm_unet* h, int B, int H, int W, int training) {
     UnetEngine& e = h->e;
+    ++h->graph_epoch;                  // the dry plan clears the op lists
     e.P = nullptr; e.G = nullptr; e.ws = nullptr; e.planned = false;
     e.zf_cursor = e.zb_cursor = 0;
     const int rc = e.plan(B, H, W, training != 0, true);
@@ -592,6 +597,7 @@ long long ddpm_unet_workspace_bytes(ddpm_unet* h, int B, int H, int W, int train
 }
 int ddpm_unet_plan(ddpm_unet* h, int B, int H, int W, int training, float* params_flat, float* grads_flat, void* workspace, long long workspace_bytes) {
     UnetEngine& e = h->e;
+    ++h->graph_epoch;
     if (!params_flat || !workspace) return fail(-30, "params / workspace pointer is null");
     if (training && !grads_flat) return fail(-30, "training plan needs a gradient buffer");
     int rc = ddpm_runtime_check(); if (rc) return rc;
@@ -674,17 +680,23 @@ int ddpm_train_backward(ddpm_unet* h, const float* gscale, void* stream) {
     return e.run_list(e.bwd_ops, st);
 }
 
+// Size a step table the handle owns for n steps.  A captured graph holds the table's address: the same length keeps the allocation
+// (rewritten in place by the caller), a new one reallocates it and moves the graph epoch.
+static int size_table(ddpm_unet* h, void*& table, int& len, int n, size_t bytes) {
+    if (len == n) return 0;
+    if (table) { cudaFree(table); table = nullptr; len = 0; }
+    ++h->graph_epoch;
+    DDPM_CUDA_OK(cudaMalloc(&table, bytes));
+    len = n;
+    return 0;
+}
 int ddpm_sampler_setup(ddpm_unet* h, int S, const int64_t* t_model_host, const float* coef_host) {
     if (!h || S <= 0) return fail(-30, "bad sampler setup");
-    if (h->S != S) {           // same length: keep the allocations (a captured sampler graph holds their addresses)
-        if (h->d_tmodel) { cudaFree(h->d_tmodel); h->d_tmodel = nullptr; }
-        if (h->d_coef) { cudaFree(h->d_coef); h->d_coef = nullptr; }
-        DDPM_CUDA_OK(cudaMalloc(&h->d_tmodel, (size_t)S * 8));
-        DDPM_CUDA_OK(cudaMalloc(&h->d_coef, (size_t)S * 6 * 4));
-    }
-    DDPM_CUDA_OK(cudaMemcpy(h->d_tmodel, t_model_host, (size_t)S * 8, cudaMemcpyHostToDevice));
-    DDPM_CUDA_OK(cudaMemcpy(h->d_coef, coef_host, (size_t)S * 6 * 4, cudaMemcpyHostToDevice));
-    h->S = S;
+    const int rc = size_table(h, h->d_samp, h->S, S, (size_t)S * 8 + (size_t)S * 6 * 4);
+    if (rc) return rc;
+    long long* tm = static_cast<long long*>(h->d_samp);
+    DDPM_CUDA_OK(cudaMemcpy(tm, t_model_host, (size_t)S * 8, cudaMemcpyHostToDevice));
+    DDPM_CUDA_OK(cudaMemcpy(tm + S, coef_host, (size_t)S * 6 * 4, cudaMemcpyHostToDevice));
     return 0;
 }
 int ddpm_sampler_reset(ddpm_unet* h, int first_step, void* stream) {
@@ -701,12 +713,13 @@ int ddpm_sampler_step_pred(ddpm_unet* h, float* x, const float* z, uint64_t seed
     // the step updates x_t in place from eps: both must have the image's channel count
     if (h && h->e.cfg.in_channels != h->e.cfg.out_channels) return fail(-30, "ddpm_sampler_step: eps prediction needs out_channels == in_channels");
     NEED_PLAN(h);
-    if (!h->d_coef) return fail(-33, "ddpm_sampler_setup has not been called");
+    if (!h->d_samp) return fail(-33, "ddpm_sampler_setup has not been called");
     UnetEngine& e = h->e;
     h->temb_rows = false;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     long long* tbuf = e.at<long long>(e.tbuf_off); float* cc = e.at<float>(e.coefcur_off); float* eps = e.at<float>(e.eps_off);
-    launch_k(k_sampler_prep, 1, 256, 0, st, e.at<int>(e.counter_off), h->d_tmodel, h->d_coef, 6, tbuf, cc, e.B);
+    const long long* tm = static_cast<const long long*>(h->d_samp);
+    launch_k(k_sampler_prep, 1, 256, 0, st, e.at<int>(e.counter_off), tm, reinterpret_cast<const float*>(tm + h->S), 6, tbuf, cc, e.B);
     DDPM_CUDA_OK(cudaGetLastError());
     e.x_in = x; e.t_in = tbuf; e.eps_dst = eps; e.drop_seed = 0;
     static const bool no_uni = getenv("DDPM_NO_UNIFORM_T") != nullptr;
@@ -740,12 +753,9 @@ int ddpm_bpd_setup(ddpm_unet* h, int T, const float* coef_host) {
         ta[i] = coef_host[(size_t)i * kBpdRow + 0];       // the q_sample prologue indexes its tables by t
         ts[i] = coef_host[(size_t)i * kBpdRow + 1];
     }
-    if (h->bpd_T != T) {       // same length: keep the allocation (a captured bits/dim graph holds its address)
-        if (h->d_bpd) { cudaFree(h->d_bpd); h->d_bpd = nullptr; h->bpd_T = 0; }
-        DDPM_CUDA_OK(cudaMalloc(&h->d_bpd, bytes));
-    }
+    const int rc = size_table(h, h->d_bpd, h->bpd_T, T, bytes);
+    if (rc) return rc;
     DDPM_CUDA_OK(cudaMemcpy(h->d_bpd, host.data(), bytes, cudaMemcpyHostToDevice));
-    h->bpd_T = T;
     return 0;
 }
 int ddpm_bpd_reset(ddpm_unet* h, int first_step, void* stream) {

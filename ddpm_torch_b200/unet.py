@@ -87,9 +87,7 @@ class UNet(nn.Module):
         self._packed_version = None
         self._packed_epoch = 0
         self._drop_calls = 0
-        self._plan_epoch = 0
         self._sampler_cache = {}
-        self._bpd_T, self._bpd_gen = 0, 0    # chain length of the handle's bits/dim table and its allocation generation
         self._acc = None                   # gradient-accumulation buffer (only exists when backward runs twice before a step)
         self._acc_pending = False
         self._bwd_since_zero = 0
@@ -180,26 +178,13 @@ class UNet(nn.Module):
                                "move the model with .cuda() first")
         if not self._views_ok():
             self._reflatten()
-        L = _lib.lib()
         key = (B, H, W, bool(training), self._flat.data_ptr())
         if key != self._plan_key:
-            need = L.ddpm_unet_workspace_bytes(self._h, B, H, W, int(training))
-            if need < 0:
-                _lib.check(int(need), "workspace_bytes")
             dev = self._flat.device
-            if self._ws is None or self._ws.numel() < need or self._ws.device != dev:
-                if self._ws is not None:
-                    torch.cuda.synchronize(self._ws.device)     # the engine's side stream may still hold a queued weight re-pack into it
-                self._ws = None
-                self._ws = torch.empty(int(need), dtype=torch.uint8, device=dev)
             if training and (self._grads is None or self._grads.device != dev):
                 self._grads = torch.zeros(self._flat_elems, dtype=torch.float32, device=dev)
-            with torch.cuda.device(dev):
-                _lib.check(L.ddpm_unet_plan(self._h, B, H, W, int(training), self._flat.data_ptr(),
-                                            self._grads.data_ptr() if training else None,
-                                            self._ws.data_ptr(), self._ws.numel()), "unet_plan")
+            self._ws = self._plan(self._h, self._ws, B, H, W, self._grads if training else None)
             self._plan_key = key
-            self._plan_epoch += 1                 # captured sampler graphs of older plans are stale (see diffusion._native_sample_loop)
             self._packed_version = None
         self.repack_if_needed(force=training or force_repack)
         return self._h
@@ -212,30 +197,38 @@ class UNet(nn.Module):
             raise RuntimeError("ddpm_torch_b200.UNet runs on sm_90a CUDA devices only (no CPU / PyTorch fallback)")
         if not self._views_ok():
             self._reflatten()
-        L = _lib.lib()
         a = self._aux.get(idx)
+        if a is None:
+            h = C.c_void_p()
+            _lib.check(_lib.lib().ddpm_unet_create_ex(C.byref(self._cfg), int(self.resample_with_conv), C.byref(h)), "unet_create")
+            a = self._aux[idx] = {"h": h, "ws": None, "key": None, "ver": None}
         key = (B, H, W, self._flat.data_ptr())
-        if a is None or a["key"] != key:
-            if a is None:
-                h = C.c_void_p()
-                _lib.check(L.ddpm_unet_create_ex(C.byref(self._cfg), int(self.resample_with_conv), C.byref(h)), "unet_create")
-                a = {"h": h, "ws": None, "key": None, "ver": None}
-                self._aux[idx] = a
-            need = L.ddpm_unet_workspace_bytes(a["h"], B, H, W, 0)
-            if need < 0:
-                _lib.check(int(need), "workspace_bytes")
-            if a["ws"] is None or a["ws"].numel() < need or a["ws"].device != self._flat.device:
-                a["ws"] = None
-                a["ws"] = torch.empty(int(need), dtype=torch.uint8, device=self._flat.device)
-            with torch.cuda.device(self._flat.device):
-                _lib.check(L.ddpm_unet_plan(a["h"], B, H, W, 0, self._flat.data_ptr(), None, a["ws"].data_ptr(), a["ws"].numel()), "unet_plan")
+        if a["key"] != key:
+            a["ws"] = self._plan(a["h"], a["ws"], B, H, W)
             a["key"], a["ver"] = key, None
-            a["epoch"] = a.get("epoch", 0) + 1
         if force or a["ver"] != self._weights_version():
             with torch.cuda.device(self._flat.device):
-                _lib.check(L.ddpm_unet_repack(a["h"], _lib.stream_ptr(self._flat.device)), "unet_repack")
+                _lib.check(_lib.lib().ddpm_unet_repack(a["h"], _lib.stream_ptr(self._flat.device)), "unet_repack")
             a["ver"] = self._weights_version()
         return a["h"]
+
+    def _plan(self, h, ws, B, H, W, grads=None):
+        """Compile handle ``h``'s launch plan for a (B, H, W) batch over the flat parameters: a training plan writing ``grads``
+        when that flat gradient buffer is given, an inference plan otherwise.  Returns the workspace the plan is bound to:
+        ``ws`` when it is large enough and on the parameters' device, else a new one."""
+        L = _lib.lib()
+        need = L.ddpm_unet_workspace_bytes(h, B, H, W, int(grads is not None))
+        if need < 0:
+            _lib.check(int(need), "workspace_bytes")
+        dev = self._flat.device
+        if ws is None or ws.numel() < need or ws.device != dev:
+            if ws is not None:
+                torch.cuda.synchronize(ws.device)     # the engine's side stream may still hold a queued weight re-pack into it
+            ws = torch.empty(int(need), dtype=torch.uint8, device=dev)
+        with torch.cuda.device(dev):
+            _lib.check(L.ddpm_unet_plan(h, B, H, W, int(grads is not None), self._flat.data_ptr(),
+                                        None if grads is None else grads.data_ptr(), ws.data_ptr(), ws.numel()), "unet_plan")
+        return ws
 
     def repack_if_needed(self, force=False):
         v = self._weights_version()

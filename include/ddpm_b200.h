@@ -298,6 +298,11 @@ void ddpm_unet_destroy(ddpm_unet* h);
 int       ddpm_unet_num_params(const ddpm_unet* h);
 int       ddpm_unet_param_info(const ddpm_unet* h, int i, const char** name, int* ndim, int dims[4], long long* offset);
 long long ddpm_unet_flat_elems(const ddpm_unet* h);
+/* Graph validity: a CUDA graph captured from this handle's launches stays valid while the value returned here is unchanged.
+ * It moves on every ddpm_unet_workspace_bytes and ddpm_unet_plan call (both rebuild the launch lists) and whenever
+ * ddpm_sampler_setup or ddpm_bpd_setup reallocates its table for a new length; a setup with the same length rewrites the table
+ * in place and leaves it unchanged.  A null handle returns a negative error code. */
+long long ddpm_unet_graph_epoch(const ddpm_unet* h);
 /* Workspace bytes for a (batch, H, W) plan; training != 0 also plans the backward pass. */
 long long ddpm_unet_workspace_bytes(ddpm_unet* h, int B, int H, int W, int training);
 /* Bind caller-owned device buffers and compile the launch plan. grads_flat may be NULL when training == 0. */

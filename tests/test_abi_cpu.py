@@ -126,6 +126,18 @@ def test_bad_configs_return_errors_not_aborts(L):
     L.ddpm_unet_destroy(h)
 
 
+def test_graph_epoch_moves_with_every_dry_plan(L):
+    h = _handle(L, R.TINY_CFG)
+    e = L.ddpm_unet_graph_epoch(h)
+    assert e >= 0, L.ddpm_last_error()
+    for _ in range(2):
+        assert L.ddpm_unet_workspace_bytes(h, 2, 16, 16, 0) > 0
+        assert L.ddpm_unet_graph_epoch(h) > e
+        e = L.ddpm_unet_graph_epoch(h)
+    assert L.ddpm_unet_graph_epoch(None) < 0 and b"null" in L.ddpm_last_error()
+    L.ddpm_unet_destroy(h)
+
+
 def test_python_module_mirrors_reference_surface():
     import inspect
     import ddpm_torch_b200 as D

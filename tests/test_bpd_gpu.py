@@ -7,7 +7,7 @@
    B = 4, T = 1000, same ``torch.manual_seed``: the epilogue repeats the torch operations in order, so only the per-image
    reduction order and the forward's own run-to-run drift differ - per term rtol 1e-3 / atol 1e-5 bits, total relative
    <= 1e-4 (mses: rtol 1e-2, see the test).
-3. Graph replay vs eager launches, and two batch sizes one after the other on one model.
+3. Graph replay vs eager launches, with two batch sizes and two chain lengths (T = 20 -> 10 -> 20) one after the other on one model.
 4. A reference-EMA ``.data.copy_`` weight swap between two calls is seen; train/eval mode is restored."""
 import pytest
 import torch
@@ -103,14 +103,15 @@ def test_native_bpd_matches_generic_loop_on_same_engine(vt, clip):
 
 def test_graph_replay_equals_eager_and_ragged_batches_run():
     m = build(R.SMALL64_CFG, 3)
-    d = diffusion(20, "fixed-large")
-    for B in (4, 3, 4):
+    ds = {T: diffusion(T, "fixed-large") for T in (20, 10)}
+    for T, B in ((20, 4), (20, 3), (20, 4), (10, 4), (20, 4)):      # a new T at one shape reallocates the handle's step table
+        d = ds[T]
         x0 = data(B, 32, 10 + B)
         torch.manual_seed(99)
         gr = d.calc_all_bpd(m, x0, use_graph=True)
         torch.manual_seed(99)
         ea = d.calc_all_bpd(m, x0, use_graph=False)
-        assert gr[1].shape == (B, 20) and gr[0].shape == (B,)
+        assert gr[1].shape == (B, T) and gr[0].shape == (B,)
         torch.testing.assert_close(gr[1], ea[1], rtol=1e-3, atol=1e-5)
         torch.testing.assert_close(gr[3], ea[3], rtol=1e-3, atol=1e-5)
         assert ((gr[0] - ea[0]).abs() / ea[0].abs()).max().item() <= 1e-4

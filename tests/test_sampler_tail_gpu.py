@@ -7,7 +7,8 @@ then + bias; CUDA-core k_out_conv: bias + sum a * 0).  What remains is the step 
           and pred_x0 must equal the mirror's, run on the CPU with denoise_fn = BETA and the same z, BIT FOR BIT.
   chains  p_sample (DDPM, T = 20, both variances; DDIM on 20 of 1000 steps with eta in {0, 0.5, 1}), graph and eager, split 1 and
           2, against the mirror's CPU loop fed the same torch.Generator stream: bit-identical at the end.  This checks
-          k_sampler_prep's counter walk and row selection.
+          k_sampler_prep's counter walk and row selection.  Also DDPM T = 20 and DDIM on 10 steps alternating on one model: a
+          new chain length captures a new step graph, the same length replays the cached one.
   philox  rng = "philox" with BETA = 0 and x_t = 0 writes x_{t-1} = fl(sigma z): z at CIFAR-10 shape, B = 256 (786k samples per
           step), fixed seeds.  Mean and variance within 5 sigma of N(0, 1), KS p > 1e-3, |z| <= sqrt(-2 ln 2^-32) (u1 >= 2^-32;
           1e-5 relative for __logf and the division by sigma), correlation of consecutive steps and of the two split halves' seeds
@@ -133,21 +134,39 @@ def mirror_chain(diff, x_T, seed, fn):
     return x
 
 
-@pytest.mark.parametrize("kind", ["ddpm-large", "ddpm-small", "ddim0", "ddim0.5", "ddim1"])
-def test_chains_bit_exact(kind):
+def chain(kind):
+    """ddpm-large / ddpm-small: DDPM with T = 20; ddim<eta>[/<S>]: DDIM on S (default 20) of 1000 steps"""
     from ddpm_torch_b200.ddim import DDIM, get_selection_schedule
-    m, HW = model("small64")
     if kind.startswith("ddpm"):
-        diff = diffusion("fixed-large" if kind.endswith("large") else "fixed-small", T=20)
-    else:
-        diff = DDIM.from_ddpm(diffusion("fixed-large"), eta=float(kind[4:]), subsequence=get_selection_schedule("linear", 20, 1000))
+        return diffusion("fixed-large" if kind.endswith("large") else "fixed-small", T=20)
+    eta, _, S = kind[4:].partition("/")
+    return DDIM.from_ddpm(diffusion("fixed-large"), eta=float(eta), subsequence=get_selection_schedule("linear", int(S or 20), 1000))
+
+
+# chains run in order on one model: each change of chain length reallocates the handles' step tables, so the step graph cached
+# by the previous call of that length must be captured anew rather than replayed; DDIM with a new eta keeps the length and the graph
+REALLOC = ("ddpm-large", "ddim0/10", "ddpm-large", "ddim0/10", "ddim1/10")
+
+
+@pytest.mark.parametrize("kinds", [(k,) for k in ("ddpm-large", "ddpm-small", "ddim0", "ddim0.5", "ddim1")] + [REALLOC], ids=",".join)
+def test_chains_bit_exact(kinds):
+    m, HW = model("small64")
     B = 4
     x_T = torch.randn(B, 3, HW, HW, generator=torch.Generator().manual_seed(3))
-    ref = mirror_chain(diff, x_T, 11, pinned_fn())
+    diffs = [chain(k) for k in kinds]
+    refs = [mirror_chain(diff, x_T, 11, pinned_fn()) for diff in diffs]
     for use_graph in (True, False):
         for split in (1, 2):
-            out = diff.p_sample(m, (B, 3, HW, HW), device=DEV, noise=x_T.to(DEV), seed=11, use_graph=use_graph, split=split)
-            assert torch.equal(out.cpu(), ref), f"{kind} graph={use_graph} split={split}: max {(out.cpu() - ref).abs().max():.3e}"
+            for j, (kind, diff, ref) in enumerate(zip(kinds, diffs, refs)):
+                before = {k: e["graph"] for k, e in m._sampler_cache.items()}
+                out = diff.p_sample(m, (B, 3, HW, HW), device=DEV, noise=x_T.to(DEV), seed=11, use_graph=use_graph, split=split)
+                assert torch.equal(out.cpu(), ref), f"{kind} graph={use_graph} split={split}: max {(out.cpu() - ref).abs().max():.3e}"
+                if use_graph:
+                    new = [e["graph"] for k, e in m._sampler_cache.items() if k not in before]
+                    recapture = j == 0 or len(diffs[j - 1].betas) != len(diff.betas)
+                    assert len(new) == int(recapture), f"{kind} split={split}: {len(new)} graphs captured"
+                    assert all(g is not old for g in new for old in before.values())
+                    assert all(m._sampler_cache[k]["graph"] is g for k, g in before.items() if k in m._sampler_cache)
     assert L().ddpm_device_error_flag() == 0
 
 
