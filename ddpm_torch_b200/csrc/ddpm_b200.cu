@@ -23,6 +23,7 @@ struct ddpm_unet {
     const float* train_target = nullptr;
     bool temb_rows = false;        // the last forward of this plan was a per-row ddpm_unet_temb_forward (what its backward reads);
                                    // every other forward entry point clears it
+    bool image_fwd = false;        // the last forward of this plan was a ddpm_unet_image_forward (what its backward reads); cleared likewise
 };
 
 __global__ void k_set_int(int* p, int v) {
@@ -601,7 +602,7 @@ int ddpm_unet_plan(ddpm_unet* h, int B, int H, int W, int training, float* param
     if (!params_flat || !workspace) return fail(-30, "params / workspace pointer is null");
     if (training && !grads_flat) return fail(-30, "training plan needs a gradient buffer");
     int rc = ddpm_runtime_check(); if (rc) return rc;
-    e.planned = false; h->temb_rows = false;
+    e.planned = false; h->temb_rows = false; h->image_fwd = false;
     e.P = params_flat; e.G = grads_flat; e.ws = static_cast<uint8_t*>(workspace); e.ws_bytes = (size_t)workspace_bytes;
     e.zf_cursor = e.zb_cursor = 0;
     if ((rc = e.plan(B, H, W, training != 0, true))) return rc;
@@ -618,7 +619,7 @@ int ddpm_unet_repack(ddpm_unet* h, void* stream) { NEED_PLAN(h); return h->e.rep
 int ddpm_unet_forward(ddpm_unet* h, const float* x, const int64_t* t, float* eps, uint64_t dropout_seed, void* stream) {
     NEED_PLAN(h);
     UnetEngine& e = h->e;
-    h->temb_rows = false;
+    h->temb_rows = false; h->image_fwd = false;
     e.x_in = x; e.t_in = reinterpret_cast<const long long*>(t); e.eps_dst = eps; e.drop_seed = dropout_seed;
     return e.run_list(e.fwd_ops, static_cast<cudaStream_t>(stream));
 }
@@ -648,7 +649,7 @@ int ddpm_train_forward(ddpm_unet* h, const float* x0, const int64_t* t, const fl
     if (h && h->e.cfg.in_channels != h->e.cfg.out_channels) return fail(-30, "ddpm_train_forward: eps prediction needs out_channels == in_channels");
     NEED_PLAN(h);
     UnetEngine& e = h->e;
-    h->temb_rows = false;
+    h->temb_rows = false; h->image_fwd = false;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int per_img = e.cfg.in_channels * e.H * e.W;
     const long long total = (long long)e.B * per_img;
@@ -715,7 +716,7 @@ int ddpm_sampler_step_pred(ddpm_unet* h, float* x, const float* z, uint64_t seed
     NEED_PLAN(h);
     if (!h->d_samp) return fail(-33, "ddpm_sampler_setup has not been called");
     UnetEngine& e = h->e;
-    h->temb_rows = false;
+    h->temb_rows = false; h->image_fwd = false;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     long long* tbuf = e.at<long long>(e.tbuf_off); float* cc = e.at<float>(e.coefcur_off); float* eps = e.at<float>(e.eps_off);
     const long long* tm = static_cast<const long long*>(h->d_samp);
@@ -772,7 +773,7 @@ int ddpm_bpd_step(ddpm_unet* h, const float* x0, const float* noise, int clip_de
     NEED_PLAN(h);
     if (!h->d_bpd) return fail(-33, "ddpm_bpd_setup has not been called");
     UnetEngine& e = h->e;
-    h->temb_rows = false;
+    h->temb_rows = false; h->image_fwd = false;
     const int Cin = e.cfg.in_channels, Cout = e.cfg.out_channels, HW = e.H * e.W, T = h->bpd_T;
     if (Cin != Cout) return fail(-30, "ddpm_bpd_step: eps prediction needs out_channels == in_channels");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -917,7 +918,7 @@ int ddpm_unet_temb_forward(ddpm_unet* h, const int64_t* t, int uniform, float* e
     if (uniform) ops.insert(ops.end(), e.temb_uni_ops.begin(), e.temb_uni_ops.end());
     else for (const Op& o : e.fwd_ops) if (o.tag == OP_TEMB) ops.push_back(o);
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    h->temb_rows = false;
+    h->temb_rows = false; h->image_fwd = false;
     e.t_in = reinterpret_cast<const long long*>(t);
     int rc = e.run_list(ops, st);           // honours Op::wait_pack: the tensor-core projection waits for a pending repack
     if (rc) return rc;
@@ -954,6 +955,90 @@ int ddpm_unet_temb_backward(ddpm_unet* h, const float* dtp, float* d_st, float* 
     if (d_st) DDPM_CUDA_OK(cudaMemcpyAsync(d_st, e.temb.d_st, (size_t)e.B * e.temb.E * 4, cudaMemcpyDefault, st));
     if (d_s0) DDPM_CUDA_OK(cudaMemcpyAsync(d_s0, e.temb.d_s0, (size_t)e.B * e.temb.E * 4, cudaMemcpyDefault, st));
     return 0;
+}
+
+// ------------------------------------------------------------------------------------------------ image-side convolution probes
+int ddpm_unet_image_layout(const ddpm_unet* h, int* in_route, int* in_wgrad_route, int* out_route, int* dx_route, int* h0_qstats) {
+    if (!h) return fail(-30, "ddpm_unet_image_layout: null handle");
+    const UnetEngine& e = h->e;
+    if (e.img.in_tc < 0 || e.img.out_tc < 0) return fail(-33, "ddpm_unet_image_layout: no plan (ddpm_unet_workspace_bytes or ddpm_unet_plan first)");
+    if (in_route) *in_route = e.img.in_tc;
+    if (in_wgrad_route) *in_wgrad_route = e.img.in_wgrad_tc;
+    if (out_route) *out_route = e.img.out_tc;
+    if (dx_route) *dx_route = e.img.dx_tc;
+    if (h0_qstats) *h0_qstats = e.img.h0_qs ? 1 : 0;
+    return 0;
+}
+
+// the ops of `L` whose names start with `prefix` (and run for this variant of the backward), in plan order
+static std::vector<Op> ops_named(const std::vector<Op>& L, const std::string& prefix, bool want_dx = false) {
+    std::vector<Op> r;
+    for (const Op& o : L) if (o.name.compare(0, prefix.size(), prefix) == 0 && o.runs(want_dx, true)) r.push_back(o);
+    return r;
+}
+
+int ddpm_unet_image_forward(ddpm_unet* h, const float* x, const int64_t* t, const float* noise, const float* tab_a, const float* tab_s,
+                            const void* a, float* xt_out, void* h0_out, double* h0_qstats_out, float* eps_out, void* stream) {
+    if (!h) return fail(-30, "ddpm_unet_image_forward: null handle");
+    if (!x || !a || !eps_out) return fail(-30, "ddpm_unet_image_forward: x, a and eps_out are required");
+    if (noise && (!t || !tab_a || !tab_s)) return fail(-30, "ddpm_unet_image_forward: noise needs t, tab_a and tab_s");
+    if (xt_out && !noise) return fail(-30, "ddpm_unet_image_forward: xt_out needs noise (x_t is formed by the q_sample prologue)");
+    NEED_PLAN(h);
+    UnetEngine& e = h->e;
+    if (h0_qstats_out && !e.img.h0_qs) return fail(-30, "ddpm_unet_image_forward: this plan computes no quad statistics of h0");
+    // the forward's zero op and in_conv's ops; then out_conv.2's, which wait for a pending repack as the forward's first consumer
+    // of packed weights does
+    std::vector<Op> in_ops, out_ops = ops_named(e.fwd_ops, "out_conv.2");
+    for (const Op& o : e.fwd_ops) if (o.name == "zero.fwd") in_ops.push_back(o);
+    for (const Op& o : ops_named(e.fwd_ops, "in_conv")) in_ops.push_back(o);
+    if (in_ops.size() < 2 || out_ops.empty()) return fail(-31, "ddpm_unet_image_forward: internal: image ops not found");
+    out_ops.front().wait_pack = 2;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    h->temb_rows = false; h->image_fwd = false;
+    float* xt = e.at<float>(e.xt_off);
+    if (noise) e.qs_pro = QsamplePro{noise, reinterpret_cast<const long long*>(t), tab_a, tab_s, xt};
+    e.x_in = x;
+    int rc = e.run_list(in_ops, st);
+    e.qs_pro = QsamplePro{};
+    e.x_in = noise ? xt : x;                           // what the backward reads as the network input, as after ddpm_train_forward
+    if (rc) return rc;
+    const size_t P = (size_t)e.B * e.H * e.W, ch = (size_t)e.cfg.hid_channels;
+    DDPM_CUDA_OK(cudaMemcpyAsync(e.img.a, a, P * ch * 2, cudaMemcpyDefault, st));
+    e.eps_dst = eps_out;
+    if ((rc = e.run_list(out_ops, st))) return rc;
+    if (xt_out) DDPM_CUDA_OK(cudaMemcpyAsync(xt_out, xt, P * e.cfg.in_channels * 4, cudaMemcpyDefault, st));
+    if (h0_out) DDPM_CUDA_OK(cudaMemcpyAsync(h0_out, e.img.h0, P * ch * 2, cudaMemcpyDefault, st));
+    if (h0_qstats_out) DDPM_CUDA_OK(cudaMemcpyAsync(h0_qstats_out, e.img.h0_qs, (size_t)e.B * (ch / 4) * 2 * 8, cudaMemcpyDefault, st));
+    h->image_fwd = true;
+    return 0;
+}
+
+int ddpm_unet_image_backward(ddpm_unet* h, const float* d_eps, const void* dh0, float* dx_out, void* d_a_out, void* stream) {
+    if (!h) return fail(-30, "ddpm_unet_image_backward: null handle");
+    if (!d_eps || !dh0) return fail(-30, "ddpm_unet_image_backward: d_eps and dh0 are required");
+    NEED_PLAN(h);
+    UnetEngine& e = h->e;
+    if (!e.train) return fail(-33, "ddpm_unet_image_backward: plan was built without training");
+    if (!h->image_fwd) return fail(-33, "ddpm_unet_image_backward: needs a ddpm_unet_image_forward of this plan first");
+    // the backward's zero op (accumulators + the flat gradient buffer), out_conv.2's backward ops; dh0 in place of what the first
+    // ResBlocks deposit, then in_conv's (with dx_out: and the input-gradient ops)
+    std::vector<Op> zero, out_ops = ops_named(e.bwd_ops, "out_conv.2"), in_ops = ops_named(e.bwd_ops, "in_conv", dx_out != nullptr);
+    for (const Op& o : e.bwd_ops) if (o.name == "zero.bwd") zero.push_back(o);
+    if (zero.size() != 1 || out_ops.empty() || in_ops.empty() || !e.img.d_a || !e.img.dh0)
+        return fail(-31, "ddpm_unet_image_backward: internal: image ops not found");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const size_t P = (size_t)e.B * e.H * e.W, ch = (size_t)e.cfg.hid_channels;
+    e.bwd_params = true; e.bwd_dx = dx_out != nullptr; e.dx_dst = dx_out; e.deps_src = d_eps;
+    auto run = [&]() -> int {                           // each run_list joins the side stream (weight gradients, unpacks, bias sums)
+        int rc = e.run_list(zero, st);
+        if (rc || (rc = e.run_list(out_ops, st))) return rc;
+        if (d_a_out) DDPM_CUDA_OK(cudaMemcpyAsync(d_a_out, e.img.d_a, P * ch * 2, cudaMemcpyDefault, st));
+        DDPM_CUDA_OK(cudaMemcpyAsync(e.img.dh0, dh0, P * ch * 2, cudaMemcpyDefault, st));
+        return e.run_list(in_ops, st);
+    };
+    const int rc = run();
+    e.dx_dst = nullptr; e.bwd_dx = false;
+    return rc;
 }
 
 // ------------------------------------------------------------------------------------------------ 2-D toy denoiser (toy_mlp.cuh)

@@ -593,6 +593,11 @@ struct UnetEngine {
     struct TembBufs { float *emb = nullptr, *e0 = nullptr, *e1 = nullptr, *TP = nullptr, *dTP = nullptr, *d_st = nullptr, *d_s0 = nullptr;
                       int E = 0, tp_ld = 0, maxc = 0; bool tc = false; } temb;
     std::vector<std::string> tp_block_host;
+    // the image-side convolutions as planned (read by the ddpm_unet_image_* probes): routes 1 = tensor cores, 0 = CUDA cores,
+    // -1 = not in this plan (weight gradient and dx of an inference plan); h0 and its quad statistics, out_conv.0's output a,
+    // and the gradients d_a (of a) and dh0 (of h0)
+    struct ImgBufs { int in_tc = -1, in_wgrad_tc = -1, out_tc = -1, dx_tc = -1;
+                     bf16 *h0 = nullptr, *a = nullptr, *d_a = nullptr, *dh0 = nullptr; double* h0_qs = nullptr; } img;
     uint32_t layer_counter = 0;
     double fwd_flops = 0, bwd_flops = 0;
     int n_tc_gemms = 0, n_generic = 0;

@@ -276,7 +276,7 @@ inline int UnetEngine::plan(int B_, int H_, int W_, bool train_, bool dry_) {
     cursor = 0; pack_ops.clear(); fwd_ops.clear(); bwd_ops.clear(); tape.clear(); tape_tag.clear(); cur_tag = "late"; grads.clear(); once_list.clear();
     { std::vector<GradChunk> keep; keep.swap(chunks); for (auto& c : keep) if (c.ev) cudaEventDestroy(c.ev); }
     tp_table_host.clear(); tp_uni_table_host.clear(); fc_table_host.clear(); tpw_table_host.clear(); tpd_table_host.clear(); pack_table_host.clear(); unpack_table_host.clear();
-    tp_block_host.clear(); temb = TembBufs{};
+    tp_block_host.clear(); temb = TembBufs{}; img = ImgBufs{};
     layer_counter = 0; fwd_flops = bwd_flops = 0; n_tc_gemms = n_generic = 0; plan_error = 0; gather_fused_tail = false; out_T = nullptr;
     const size_t zf_total = zf_cursor, zb_total = zb_cursor;   // sizes learned by the preceding dry pass
     zf_cursor = zb_cursor = 0;
@@ -516,15 +516,18 @@ inline int UnetEngine::plan(int B_, int H_, int W_, bool train_, bool dry_) {
             return (int)cudaGetLastError(); });
         fwd_flops += 2.0 * B * H * W * ch * Cin * 9;
         first_packed_op = fwd_ops.size();          // in_conv reads the fp32 master weights; everything after it reads packed ones
+        img.in_tc = tc_in ? 1 : 0; img.h0 = o; img.h0_qs = h0.qs >= 0 ? at<double>((size_t)h0.qs) : nullptr;
         if (train) tape_push([=]() {
             const T4 dY = grad_of(h0, nullptr);
             float* gw = GP("in_conv.weight"); float* gb = GP("in_conv.bias"); const bf16* d = bp(dY);
+            self->img.dh0 = bp(dY);
             const long long P = (long long)Bn * Hn * Wn; const int ppb = 256; const int nb = (int)((P + ppb - 1) / ppb);
             bwd_flops += 2.0 * P * ch * Cin * 9;
             const long long s_c = (long long)Cin * 9;
             static const bool no_tc_in = getenv("DDPM_NO_TC_OUTCONV") != nullptr;
             RoleScope role(self, ROLE_PARAM);          // the network input's gradient is the dx op at the end of the plan
-            if (!no_tc_in && ch % 64 == 0 && tc_ok_geom(H, W) && 9 * Cin <= 64) {
+            self->img.in_wgrad_tc = (!no_tc_in && ch % 64 == 0 && tc_ok_geom(H, W) && 9 * Cin <= 64) ? 1 : 0;
+            if (self->img.in_wgrad_tc) {
                 // weight gradient on the tensor cores: X = im2col(x) [P][64] bf16, S[ch][64] = dY^T x X (MN-major GEMM, side stream)
                 T4 X = tc_in ? Xcol : newT(B, H, W, 64);
                 bf16* Xp = bp(X);
@@ -606,6 +609,7 @@ inline int UnetEngine::plan(int B_, int H_, int W_, bool train_, bool dry_) {
         fwd_flops += fl;
         static const bool no_tc_out = getenv("DDPM_NO_TC_OUTCONV") != nullptr;
         bool tc_out = !no_tc_out && ch % 64 == 0 && tc_ok_geom(H, W) && 9 * Cout <= 32;
+        img.out_tc = tc_out ? 1 : 0; img.a = bp(a_out);
         bf16* w27t = nullptr;
         if (tc_out) {
             // tensor-core path: 1x1 GEMM a[P][ch] x W27[32][ch]^T -> fp32 tap outputs T[P][32], then a 9-point gather
@@ -660,6 +664,7 @@ inline int UnetEngine::plan(int B_, int H_, int W_, bool train_, bool dry_) {
                 float* gw = GP("out_conv.2.weight"); float* gb = GP("out_conv.2.bias");
                 T4 d_a = newT(B, H, W, ch);
                 bf16* dap = bp(d_a);
+                self->img.d_a = dap;
                 const size_t shm2 = (size_t)(ch * Cout * 9 + ch) * 4; const int n2 = grid_for((long long)Bn * Hn * Wn / 2, 128);
                 const long long P = (long long)Bn * Hn * Wn; const int ppb = 256; const int nb = (int)((P + ppb - 1) / ppb);
                 bwd_flops += 2.0 * fl;
@@ -794,6 +799,7 @@ inline int UnetEngine::plan(int B_, int H_, int W_, bool train_, bool dry_) {
         const double fl = 2.0 * P * ch * Cin * 9;
         const int nblk = grid_for(P), npk = (ch * Cin * 9 + 255) / 256;
         const bool tc_dx = !getenv("DDPM_NO_TC_OUTCONV") && ch % 64 == 0 && tc_ok_geom(H, W) && 9 * Cin <= 32;
+        img.dx_tc = tc_dx ? 1 : 0;
         if (tc_dx) {
             bf16* wdx = at<bf16>(alloc_once_zero((size_t)32 * ch * 2));
             float* T = out_T ? out_T : at<float>(alloc((size_t)P * 32 * 4));     // out_conv's forward scratch is dead by now

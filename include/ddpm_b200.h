@@ -395,6 +395,26 @@ int ddpm_unet_temb_forward(ddpm_unet* h, const int64_t* t, int uniform, float* e
  * in the flat gradient buffer.  Copies out d_st = dL/dSiLU(e1) and d_s0 = dL/dSiLU(e0), [B][E] each (may be NULL). */
 int ddpm_unet_temb_backward(ddpm_unet* h, const float* dtp, float* d_st, float* d_s0, void* stream);
 
+/* ---- image-side convolution probes: run a plan's own in_conv and out_conv.2 ops alone (operator-level tests of the engine).
+ * Routes of a planned (or dry-planned) handle, 1 = tensor cores, 0 = CUDA cores, -1 = not in this plan (an inference plan has no
+ * weight gradient and no dx): in_conv forward, in_conv weight gradient, out_conv.2 (forward and backward) and the input gradient
+ * dx; h0_qstats = 1 when in_conv writes h0's GroupNorm quad statistics [B][hid/4][2] fp64 {sum, sum of squares}.  Any pointer may
+ * be NULL. */
+int ddpm_unet_image_layout(const ddpm_unet* h, int* in_route, int* in_wgrad_route, int* out_route, int* dx_route, int* h0_qstats);
+/* The plan's "zero.fwd" op and its in_conv ops over x [B][Cin][H][W] fp32 (with noise set, the q_sample prologue forms
+ * x_t = tab_a[t_b]*x + tab_s[t_b]*noise as ddpm_train_forward does; noise needs t and both tables); then a [B][H][W][hid] bf16
+ * (device) copied into out_conv.0's output and the plan's out_conv.2 ops, eps_out [B][Cout][H][W] fp32, waiting for a pending
+ * repack as the forward does.  Copies out (device pointers, may be NULL) x_t [B][Cin][H][W] fp32 (needs noise), h0 [B][H][W][hid]
+ * bf16 and its quad statistics (refused on a plan without them).  x must stay valid until the matching backward. */
+int ddpm_unet_image_forward(ddpm_unet* h, const float* x, const int64_t* t, const float* noise, const float* tab_a, const float* tab_s,
+                            const void* a, float* xt_out, void* h0_out, double* h0_qstats_out, float* eps_out, void* stream);
+/* Training plans, right after a ddpm_unet_image_forward (any other forward of the plan in between is refused): the backward's
+ * "zero.bwd" op (which clears the flat gradient buffer), out_conv.2's backward ops over d_eps [B][Cout][H][W] fp32, then dh0
+ * [B][H][W][hid] bf16 (device) copied into the plan's gradient of h0 and in_conv's backward ops (with dx_out set, the input-gradient
+ * ops too: dx_out [B][Cin][H][W] fp32).  The in_conv.* and out_conv.2.* gradients land in the flat gradient buffer; d_a_out
+ * [B][H][W][hid] bf16 (may be NULL) receives the gradient of out_conv.0's output. */
+int ddpm_unet_image_backward(ddpm_unet* h, const float* d_eps, const void* dh0, float* dx_out, void* d_a_out, void* stream);
+
 /* ---- fused optimizer step over the flat fp32 buffers.
  * Replaces, per training step, nn.utils.clip_grad_norm_(params, max_norm) + Adam.step() + LambdaLR warm-up + EMA.update()
  * (utils/train.py:159-165, :300-305; train.py:128-132) = ~13 tiny kernels x 304 tensors, by two launches and no host sync.
