@@ -8,7 +8,10 @@ Prints one JSON line per measurement, each with the card name, power limit and m
     (``.cpu().numpy()``, per-batch np.cov, merge);
   * ``calc_fd``: the distance at D = 2048 on full-rank statistics, native against the CPU formula (scipy sqrtm), and their
     difference;
-  * ``--inception``: the torch Inception forward over ``rows`` images with seeded weights, the share of FID evaluation that stays;
+  * ``--inception``: the Inception forward over ``rows`` images (32 x 32, resized to 299) with seeded weights, batch ``batch``:
+    the native leg (``ddpm_inception_forward``) and the torch leg (cuDNN) in the same call, the TF32 rate of the native leg from
+    the conv FLOP count of the layer shapes, the largest per-image relative L2 difference between the legs, and the shares of a
+    FID evaluation after sampling that the statistics and the distance take next to the native forward;
   * ``--reference``: the same statistics and distance through the staged reference (oracle/_ref), SciPy's removed ``disp`` keyword
     shimmed by patching scipy.linalg in this process.
 Seeded inputs only; nothing is read or written outside ``--out-dir`` (default: a temporary directory).
@@ -168,11 +171,31 @@ def main():
         net = InceptionV3([3]).cuda().eval()
         g = torch.Generator(device="cuda").manual_seed(2)
         imgs = torch.rand(a.batch, 3, 32, 32, device="cuda", generator=g) * 2 - 1
+        n_b = -(-a.rows // a.batch)
+        # multiply-adds of every conv at the resized 299 x 299 input, from the shapes the torch module produces
+        shapes = []
+        hooks = [m.register_forward_hook(lambda m, i, o: shapes.append((m, o.shape))) for m in net.modules()
+                 if isinstance(m, torch.nn.Conv2d)]
+        net.use_engine = False
         with torch.inference_mode():
-            net(imgs)
-            n_b = -(-a.rows // a.batch)
-            _, t_inc = timed(lambda: [net(imgs) for _ in range(n_b)])
-        emit({"metric": "inception", "rows": n_b * a.batch, "batch": a.batch, "forward_s": t_inc,
+            net(imgs[:1])
+        for h in hooks:
+            h.remove()
+        flops = sum(2 * o[1] * o[2] * o[3] * m.in_channels * m.kernel_size[0] * m.kernel_size[1] for m, o in shapes) * n_b * a.batch
+        legs = {}
+        for leg in ("torch", "native"):                # same images, same call, torch first
+            net.use_engine = leg == "native"
+            with torch.inference_mode():
+                ref = net(imgs)[0]
+                _, legs[leg] = timed(lambda: [net(imgs) for _ in range(n_b)])
+                legs[leg + "_out"] = ref
+        t_inc = legs["native"]
+        diff = (legs["native_out"] - legs["torch_out"]).flatten(1).double()
+        rel = (diff.norm(dim=1) / legs["torch_out"].flatten(1).double().norm(dim=1)).max().item()
+        emit({"metric": "inception", "rows": n_b * a.batch, "batch": a.batch, "native_forward_s": legs["native"],
+              "torch_forward_s": legs["torch"], "torch_cudnn_allow_tf32": torch.backends.cudnn.allow_tf32,
+              "speedup": legs["torch"] / legs["native"], "conv_flop": flops, "native_tf32_tflops": flops / legs["native"] / 1e12,
+              "max_rel_l2_native_vs_torch": rel,
               "stats_share": min(t_nat, t_nat2) / (t_inc + min(t_nat, t_nat2) + t_fd),
               "calc_fd_share": t_fd / (t_inc + min(t_nat, t_nat2) + t_fd)})
         hub.cleanup()

@@ -109,6 +109,12 @@ class ConvDesc(C.Structure):
     ]
 
 
+class IncConvDesc(C.Structure):
+    _fields_ = [(n, C.c_int) for n in ("N", "H", "W", "Cin", "Cout", "kh", "kw", "stride", "ph", "pw", "c_off", "C_total")] + [
+        ("x", C.c_void_p), ("w", C.c_void_p), ("gamma", C.c_void_p), ("beta", C.c_void_p), ("mean", C.c_void_p), ("var", C.c_void_p),
+        ("out", C.c_void_p), ("scratch", C.c_void_p), ("scratch_bytes", C.c_longlong)]
+
+
 class UnetCfg(C.Structure):
     _fields_ = [("in_channels", C.c_int), ("hid_channels", C.c_int), ("out_channels", C.c_int),
                 ("levels", C.c_int), ("ch_mult", C.c_int * 8), ("num_res_blocks", C.c_int), ("attn", C.c_int * 8),
@@ -197,6 +203,17 @@ def lib():
             "ddpm_fid_stats_finalize": ([vp, i32, i64, i32, vp, vp, vp], i32),
             "ddpm_fid_distance_scratch_bytes": ([i32], i64),
             "ddpm_fid_distance": ([vp, vp, vp, vp, i32, vp, vp, i64, vp], i32),
+            "ddpm_inception_num_params": ([], i32),
+            "ddpm_inception_param_info": ([i32, C.POINTER(C.c_char_p), C.POINTER(i32), C.POINTER(i32 * 4), C.POINTER(i64)], i32),
+            "ddpm_inception_conv_info": ([i32, C.POINTER(i32 * 11)], i32),
+            "ddpm_inception_packed_bytes": ([], i64),
+            "ddpm_inception_pack": ([vp, vp, vp], i32),
+            "ddpm_inception_workspace_bytes": ([i32, i32, i32, i32, i32], i64),
+            "ddpm_inception_forward": ([vp, vp, i32, i32, i32, i32, i32, i32, C.POINTER(vp * 4), vp, vp, i64, vp], i32),
+            "ddpm_inception_conv_scratch_bytes": ([C.POINTER(IncConvDesc)], i64),
+            "ddpm_inception_conv_run": ([C.POINTER(IncConvDesc), vp], i32),
+            "ddpm_inception_pool_run": ([i32, vp, i32, i32, i32, i32, vp, i32, i32, vp], i32),
+            "ddpm_inception_input_run": ([vp, i32, i32, i32, i32, i32, vp, vp], i32),
             "ddpm_toy_num_params": ([vp], i64),
             "ddpm_toy_workspace_bytes": ([vp, i64, i32], i64),
             "ddpm_toy_forward": ([vp, vp, vp, vp, i64, vp, i32, vp, i64, vp], i32),
@@ -227,7 +244,10 @@ EXPORTS = ["ddpm_last_error", "ddpm_runtime_check", "ddpm_device_error_flag", "d
            "ddpm_knn_scratch_bytes", "ddpm_knn_kth", "ddpm_knn_cover",
            "ddpm_fid_stats_bytes", "ddpm_fid_stats_update", "ddpm_fid_stats_finalize", "ddpm_fid_distance_scratch_bytes",
            "ddpm_fid_distance", "ddpm_toy_num_params", "ddpm_toy_workspace_bytes", "ddpm_toy_forward", "ddpm_toy_train_forward",
-           "ddpm_toy_backward", "ddpm_toy_train_backward", "ddpm_toy_sample"]
+           "ddpm_toy_backward", "ddpm_toy_train_backward", "ddpm_toy_sample",
+           "ddpm_inception_num_params", "ddpm_inception_param_info", "ddpm_inception_conv_info", "ddpm_inception_packed_bytes", "ddpm_inception_pack",
+           "ddpm_inception_workspace_bytes", "ddpm_inception_forward", "ddpm_inception_conv_scratch_bytes", "ddpm_inception_conv_run",
+           "ddpm_inception_pool_run", "ddpm_inception_input_run"]
 
 
 def check(rc, what=""):

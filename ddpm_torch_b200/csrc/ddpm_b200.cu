@@ -8,6 +8,7 @@
 #include "optim.cuh"
 #include "knn.cuh"
 #include "fid.cuh"
+#include "inception.cuh"
 #include "toy_mlp.cuh"
 
 using namespace ddpm;
@@ -541,6 +542,175 @@ int ddpm_fid_distance(const double* mu1, const double* sigma1, const double* mu2
     if (!scratch || misaligned16(scratch) || bytes < (long long)need)
         return fail(-46, "%s: needs a 16-byte aligned scratch of ddpm_fid_distance_scratch_bytes = %zu bytes (got %lld)", fn, need, bytes);
     const cudaError_t e = fid_distance_launch(mu1, sigma1, mu2, sigma2, D, out, scratch, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? 0 : fail(-20, "%s: launch failed: %s", fn, cudaGetErrorString(e));
+}
+
+// ------------------------------------------------------------------------------------------------ FID Inception-v3 forward
+static bool misaligned(const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) != 0; }
+
+int ddpm_inception_num_params(void) { return (int)inc_params().size(); }
+
+int ddpm_inception_param_info(int i, const char** name, int* ndim, int dims[4], long long* offset) {
+    if (i < 0 || i >= (int)inc_params().size()) return fail(-47, "ddpm_inception_param_info: index %d out of 0..%d", i, (int)inc_params().size() - 1);
+    const IncParam& p = inc_params()[i];
+    if (name) *name = p.name.c_str();
+    if (ndim) *ndim = p.ndim;
+    if (dims) for (int k = 0; k < 4; ++k) dims[k] = p.dims[k];
+    if (offset) *offset = p.offset;
+    return 0;
+}
+
+int ddpm_inception_conv_info(int i, int info[11]) {
+    if (i < 0 || i >= INC_NUM_CONVS || !info) return fail(-47, "ddpm_inception_conv_info: index %d out of 0..%d or null info", i, INC_NUM_CONVS - 1);
+    static int lay[INC_NUM_CONVS][4];
+    static const int steps = [] {
+        for (auto& l : lay) l[3] = -1;
+        IncWalk w;
+        w.N = 1; w.layout = lay;
+        inc_walk(w, 299, 299, 1, 3, [](int, int, int, int, int) {});
+        return w.step;
+    }();
+    const IncConv& c = inc_convs()[i];
+    const int v[11] = {c.cin, c.cout, c.kh, c.kw, c.stride, c.ph, c.pw, lay[i][0], lay[i][1], lay[i][2], steps == INC_NUM_CONVS ? lay[i][3] : -1};
+    for (int k = 0; k < 11; ++k) info[k] = v[k];
+    return 0;
+}
+
+long long ddpm_inception_packed_bytes(void) { return inc_packed_offsets().back() * 4; }
+
+int ddpm_inception_pack(const float* raw, void* packed, void* stream) {
+    const char* fn = "ddpm_inception_pack";
+    if (!raw || misaligned(raw, 4)) return fail(-47, "%s: raw must be a non-null, 4-byte aligned fp32 buffer", fn);
+    if (!packed || misaligned(packed, 256)) return fail(-47, "%s: packed must be a non-null, 256-byte aligned buffer", fn);
+    const auto& convs = inc_convs();
+    const auto& prm = inc_params();
+    const auto& off = inc_packed_offsets();
+    float* pk = static_cast<float*>(packed);
+    for (size_t i = 0; i < convs.size(); ++i) {
+        const float* f[INC_FIELDS];
+        for (int k = 0; k < INC_FIELDS; ++k) f[k] = raw + prm[INC_FIELDS * i + k].offset;
+        const cudaError_t e = inc_fold_launch(convs[i], f[0], f[1], f[2], f[3], f[4], pk + off[2 * i], pk + off[2 * i + 1],
+                                              static_cast<cudaStream_t>(stream));
+        if (e != cudaSuccess) return fail(-20, "%s: launch failed: %s", fn, cudaGetErrorString(e));
+    }
+    return 0;
+}
+
+static int inc_check_shape(const char* fn, int N, int H, int W, int resize, int last_block) {
+    if (N < 1 || H < 1 || W < 1) return fail(-47, "%s: N, H, W must be >= 1 (got %d, %d, %d)", fn, N, H, W);
+    if ((resize != 0 && resize != 1)) return fail(-47, "%s: resize must be 0 or 1 (got %d)", fn, resize);
+    if (last_block < 0 || last_block > 3) return fail(-47, "%s: last_block must be in 0..3 (got %d)", fn, last_block);
+    if ((long long)N * 3 * H * W > INT_MAX) return fail(-47, "%s: N * 3 * H * W exceeds 2^31 - 1", fn);
+    return 0;
+}
+
+long long ddpm_inception_workspace_bytes(int N, int H, int W, int resize, int last_block) {
+    const char* fn = "ddpm_inception_workspace_bytes";
+    if (int rc = inc_check_shape(fn, N, H, W, resize, last_block)) return rc;
+    IncWalk w;
+    const char* why = nullptr;
+    const size_t b = inc_workspace(N, H, W, resize, last_block, w, why);
+    if (why) return fail(-47, "%s: %s (N %d, %d x %d, resize %d, last_block %d)", fn, why, N, H, W, resize, last_block);
+    return (long long)b;
+}
+
+int ddpm_inception_forward(const void* packed, const float* x, int N, int H, int W, int resize, int normalize, int last_block,
+                           float* const outs[4], float* pooled, void* ws, long long ws_bytes, void* stream) {
+    const char* fn = "ddpm_inception_forward";
+    if (int rc = inc_check_shape(fn, N, H, W, resize, last_block)) return rc;
+    if (normalize != 0 && normalize != 1) return fail(-47, "%s: normalize must be 0 or 1 (got %d)", fn, normalize);
+    if (!packed || misaligned(packed, 256)) return fail(-47, "%s: packed must be a non-null, 256-byte aligned buffer", fn);
+    if (!x || misaligned(x, 4)) return fail(-47, "%s: x must be a non-null, 4-byte aligned fp32 buffer", fn);
+    for (int b = 0; outs && b < 4; ++b)
+        if (outs[b] && (b > last_block || misaligned(outs[b], 4)))
+            return fail(-47, "%s: outs[%d] must be null or a 4-byte aligned buffer of a block <= last_block", fn, b);
+    if (pooled && misaligned(pooled, 4)) return fail(-47, "%s: pooled must be 4-byte aligned", fn);
+    IncWalk w;
+    const char* why = nullptr;
+    const size_t need = inc_workspace(N, H, W, resize, last_block, w, why);
+    if (why) return fail(-47, "%s: %s (N %d, %d x %d, resize %d, last_block %d)", fn, why, N, H, W, resize, last_block);
+    if (!ws || misaligned(ws, 256) || ws_bytes < (long long)need)
+        return fail(-47, "%s: needs a 256-byte aligned workspace of ddpm_inception_workspace_bytes = %zu bytes (got %lld)", fn, need, ws_bytes);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    uint8_t* p = static_cast<uint8_t*>(ws);
+    for (int b = 0; b < IncWalk::NBUF; ++b) { w.buf[b] = reinterpret_cast<float*>(p); p += inc_al256((size_t)w.need[b] * 4); }
+    w.dry = false; w.packed = static_cast<const float*>(packed); w.st = st;
+    w.err = inc_input_launch(x, N, H, W, resize, normalize, w.buf[IncWalk::X], st);
+    inc_walk(w, H, W, resize, last_block, [&](int b, int buf, int h, int wd, int C) {
+        if (!w.ok()) return;
+        const float* src = w.buf[buf];
+        const long long hw = (long long)h * wd;
+        if (b == 3) {
+            if (outs && outs[3]) w.err = launch_k(k_inc_gap, dim3(inc_grid((long long)N * C)), dim3(256), 0, st, src, N, (int)hw, C, outs[3], C);
+            if (w.ok() && pooled) w.err = launch_k(k_inc_gap, dim3(inc_grid((long long)N * C)), dim3(256), 0, st, src, N, (int)hw, C, pooled, C);
+            return;
+        }
+        if (outs && outs[b]) w.err = launch_k(k_inc_nchw, dim3(inc_grid(N * hw * C)), dim3(256), 0, st, src, N, (int)hw, C, outs[b]);
+        if (w.ok() && pooled && b == last_block)
+            w.err = launch_k(k_inc_gap, dim3(inc_grid((long long)N * C)), dim3(256), 0, st, src, N, (int)hw, C, pooled, C);
+    });
+    return w.err == cudaSuccess ? 0 : fail(-20, "%s: launch failed: %s", fn, cudaGetErrorString(w.err));
+}
+
+// the table entry a test conv stands for: any of the network's kernel shapes, with the caller's channel counts
+static int inc_conv_check(const char* fn, const ddpm_inception_conv_desc* d, IncConv& c, size_t& scratch) {
+    if (!d) return fail(-47, "%s: null descriptor", fn);
+    if (d->N < 1 || d->H < 1 || d->W < 1 || d->Cin < 1 || d->Cout < 2 || (d->Cout & 1))
+        return fail(-47, "%s: needs N, H, W, Cin >= 1 and an even Cout >= 2", fn);
+    if (d->kh < 1 || d->kw < 1 || d->kh > 7 || d->kw > 7 || d->stride < 1 || d->stride > 2 || d->ph < 0 || d->pw < 0 || d->ph >= d->kh || d->pw >= d->kw)
+        return fail(-47, "%s: kernel %d x %d, stride %d, padding (%d, %d) is outside 1..7, 1..2, 0..k-1", fn, d->kh, d->kw, d->stride, d->ph, d->pw);
+    if (d->c_off < 0 || (d->c_off & 1) || (d->C_total & 1) || d->c_off + d->Cout > d->C_total)
+        return fail(-47, "%s: channel slice [%d, %d) must be even-aligned inside an even C_total = %d", fn, d->c_off, d->c_off + d->Cout, d->C_total);
+    c = IncConv{d->Cin, d->Cout, d->kh, d->kw, d->stride, d->ph, d->pw, ""};
+    const int Ho = inc_conv_out(d->H, d->kh, d->stride, d->ph), Wo = inc_conv_out(d->W, d->kw, d->stride, d->pw);
+    if (Ho < 1 || Wo < 1) return fail(-47, "%s: empty output", fn);
+    if ((long long)d->N * d->H * d->W > INT_MAX / 4 || (long long)d->N * Ho * Wo > INT_MAX) return fail(-47, "%s: N * H * W too large", fn);
+    scratch = inc_al256((size_t)inc_cout_pad(c.cout) * inc_kp(c) * 4) + inc_al256((size_t)inc_cout_pad(c.cout) * 4);
+    return 0;
+}
+
+long long ddpm_inception_conv_scratch_bytes(const ddpm_inception_conv_desc* d) {
+    IncConv c; size_t s = 0;
+    if (int rc = inc_conv_check("ddpm_inception_conv_scratch_bytes", d, c, s)) return rc;
+    return (long long)s;
+}
+
+int ddpm_inception_conv_run(const ddpm_inception_conv_desc* d, void* stream) {
+    const char* fn = "ddpm_inception_conv_run";
+    IncConv c; size_t s = 0;
+    if (int rc = inc_conv_check(fn, d, c, s)) return rc;
+    if (!d->x || misaligned(d->x, 16)) return fail(-47, "%s: x must be a non-null, 16-byte aligned buffer", fn);
+    if (!d->w || !d->gamma || !d->beta || !d->mean || !d->var || !d->out) return fail(-47, "%s: null parameter or output", fn);
+    if (misaligned(d->out, 8)) return fail(-47, "%s: out must be 8-byte aligned", fn);
+    if (!d->scratch || misaligned(d->scratch, 256) || d->scratch_bytes < (long long)s)
+        return fail(-47, "%s: needs a 256-byte aligned scratch of ddpm_inception_conv_scratch_bytes = %zu bytes (got %lld)", fn, s, d->scratch_bytes);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    float* wp = static_cast<float*>(d->scratch);
+    float* bp = wp + inc_al256((size_t)inc_cout_pad(c.cout) * inc_kp(c) * 4) / 4;
+    cudaError_t e = inc_fold_launch(c, d->w, d->gamma, d->beta, d->mean, d->var, wp, bp, st);
+    if (e == cudaSuccess) e = inc_conv_launch(c, d->x, d->N, d->H, d->W, wp, bp, d->out, d->c_off, d->C_total, st);
+    return e == cudaSuccess ? 0 : fail(-20, "%s: launch failed: %s", fn, cudaGetErrorString(e));
+}
+
+int ddpm_inception_pool_run(int kind, const float* x, int N, int H, int W, int C, float* out, int c_off, int C_total, void* stream) {
+    const char* fn = "ddpm_inception_pool_run";
+    if (kind < 0 || kind > 2) return fail(-47, "%s: kind must be 0, 1 or 2 (got %d)", fn, kind);
+    if (N < 1 || H < 1 || W < 1 || C < 1 || (long long)N * H * W * C > INT_MAX) return fail(-47, "%s: bad shape", fn);
+    if (c_off < 0 || c_off + C > C_total) return fail(-47, "%s: channel slice outside C_total", fn);
+    int Ho, Wo;
+    inc_pool_dims(kind, H, W, Ho, Wo);
+    if (Ho < 1 || Wo < 1) return fail(-47, "%s: empty output", fn);
+    if (!x || !out || misaligned(x, 4) || misaligned(out, 4)) return fail(-47, "%s: null or misaligned buffer", fn);
+    const cudaError_t e = inc_pool_launch(kind, x, N, H, W, C, out, c_off, C_total, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? 0 : fail(-20, "%s: launch failed: %s", fn, cudaGetErrorString(e));
+}
+
+int ddpm_inception_input_run(const float* x, int N, int H, int W, int resize, int normalize, float* out, void* stream) {
+    const char* fn = "ddpm_inception_input_run";
+    if (int rc = inc_check_shape(fn, N, H, W, resize, 0)) return rc;
+    if (normalize != 0 && normalize != 1) return fail(-47, "%s: normalize must be 0 or 1 (got %d)", fn, normalize);
+    if (!x || !out || misaligned(x, 4) || misaligned(out, 16)) return fail(-47, "%s: null or misaligned buffer", fn);
+    const cudaError_t e = inc_input_launch(x, N, H, W, resize, normalize, out, static_cast<cudaStream_t>(stream));
     return e == cudaSuccess ? 0 : fail(-20, "%s: launch failed: %s", fn, cudaGetErrorString(e));
 }
 

@@ -1,5 +1,7 @@
 """FID Inception-v3 (``ddpm_torch/metrics/inception.py``): the TensorFlow FID network, assembled from torchvision's Inception
-building blocks.  Torch only: Inception runs on torch / cuDNN; only the statistics and the distance run on the engine.
+building blocks.  On an sm_90 device, with no gradient wanted and BatchNorm in eval mode, ``InceptionV3.forward`` runs on the
+engine (``ddpm_inception_forward``: TF32 tensor-core convolutions with BatchNorm folded in, csrc/inception.cuh); everything
+else (CPU, autograd, training-mode BatchNorm, ``DataParallel`` replicas, other dtypes) runs the torch modules below.
 
 The FID network differs from torchvision's ImageNet Inception-v3 in three places, all reproduced here:
   * 1008 classes (its ``fc`` is part of the checkpoint, though no feature uses it);
@@ -8,12 +10,16 @@ The FID network differs from torchvision's ImageNet Inception-v3 in three places
 Module names follow torchvision's ``Inception3``, so the published ``pt_inception-2015-12-05-6726825d.pth`` loads with
 ``strict=True``, and ``InceptionV3``'s own ``state_dict`` has the reference's ``blocks.<i>.<j>`` keys.
 """
+import ctypes as C
+import math
 import os
 
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
 import torchvision.models.inception as tvi
+
+from . import _lib
 
 FID_WEIGHTS_URL = "https://github.com/mseitzer/pytorch-fid/releases/download/fid_weights/pt_inception-2015-12-05-6726825d.pth"
 
@@ -107,8 +113,111 @@ class InceptionV3(nn.Module):
         ]
         self.blocks = nn.ModuleList(nn.Sequential(*s) for s in stages[:self.last_needed_block + 1])
         self.requires_grad_(requires_grad)
+        self.use_engine = True             # False: always the torch modules (InceptionStatistics over a device list)
+        self._native_tensors = None        # the engine's raw parameters, in its order (None: not gathered yet)
+        self._packed = None
+        self._packed_key = None
+        self._ws = None
+        self._load_epoch = 0
+        self.register_load_state_dict_post_hook(lambda module, incompatible: module._weights_changed())
+
+    def _weights_changed(self):
+        self._load_epoch += 1
+        self._packed_key = None
+
+    def _apply(self, fn, recurse=True):
+        out = super()._apply(fn, recurse)      # .to() / .cuda() may give buffers new tensors
+        self._native_tensors = None
+        self._packed_key = None
+        return out
+
+    def _engine_tensors(self):
+        """The module's conv weights and BatchNorm vectors in the engine's parameter order (ddpm_inception_param_info), or
+        None for the entries of blocks this module does not hold."""
+        if self._native_tensors is None:
+            own = dict(self.named_parameters())
+            own.update(self.named_buffers())
+            L = _lib.lib()
+            out = []
+            for i in range(L.ddpm_inception_num_params()):
+                name, ndim, dims, off = C.c_char_p(), C.c_int(), (C.c_int * 4)(), C.c_longlong()
+                _lib.check(L.ddpm_inception_param_info(i, C.byref(name), C.byref(ndim), C.byref(dims), C.byref(off)), "inception_param_info")
+                mod, rest = name.value.decode().split(".", 1)
+                key = f"{_ENGINE_BLOCK[mod]}.{rest}"
+                shape = tuple(dims[:ndim.value])
+                out.append((own.get(key), shape, off.value))
+            self._native_tensors = out
+        return self._native_tensors
+
+    def native_eligible(self, inp):
+        """True when ``forward(inp)`` runs on the engine: every parameter on one sm_90 CUDA device in fp32, BatchNorm in eval
+        mode, no gradient wanted, ``use_engine`` set, and ``inp`` a non-empty 4-D CUDA fp32 batch of 3-channel images on that
+        device.  ``DataParallel`` replicas always take the torch path."""
+        if not self.use_engine or getattr(self, "_is_replica", False) or not isinstance(inp, torch.Tensor):
+            return False
+        if not (inp.is_cuda and inp.dim() == 4 and inp.shape[0] > 0 and inp.shape[1] == 3 and inp.dtype == torch.float32):
+            return False
+        if torch.is_grad_enabled() and (inp.requires_grad or any(p.requires_grad for p in self.parameters())):
+            return False
+        if any(m.training for m in self.modules()):
+            return False
+        ts = [t for t, _, _ in self._engine_tensors() if t is not None]
+        if any(t.device != inp.device or t.dtype != torch.float32 for t in ts):
+            return False
+        return torch.cuda.get_device_capability(inp.device) == (9, 0)
+
+    def _repack_if_needed(self, dev):
+        ents = [t for t, _, _ in self._engine_tensors() if t is not None]
+        if any(t.is_inference() for t in ents):
+            key = None                         # inference tensors keep no version counter: pack on every call
+        else:
+            key = (dev, self._load_epoch, sum(t._version for t in ents), sum(t.data_ptr() for t in ents))
+        if key is not None and key == self._packed_key:
+            return
+        ents = self._engine_tensors()
+        L = _lib.lib()
+        parts = [t.detach().reshape(-1) if t is not None else torch.zeros(math.prod(shape), dtype=torch.float32, device=dev) for t, shape, _ in ents]
+        raw = torch.cat(parts)
+        if self._packed is None or self._packed.device != dev:
+            self._packed = torch.empty(L.ddpm_inception_packed_bytes(), dtype=torch.uint8, device=dev)
+        _lib.check(L.ddpm_inception_pack(raw.data_ptr(), self._packed.data_ptr(), _lib.stream_ptr(dev)), "inception_pack")
+        self._packed_key = key
+
+    def forward_native(self, inp, pooled=False):
+        """The engine's forward of ``inp`` (see ``native_eligible``): the requested blocks' outputs, NCHW fp32 as ``forward``
+        returns them; with ``pooled`` instead the [N, C] global average of the last needed block (InceptionStatistics)."""
+        dev = inp.device
+        L = _lib.lib()
+        with torch.cuda.device(dev):
+            self._repack_if_needed(dev)
+            x = inp.contiguous()
+            N, _, H, W = x.shape
+            last = self.last_needed_block
+            need = L.ddpm_inception_workspace_bytes(N, H, W, int(self.resize_input), last)
+            if need < 0:
+                _lib.check(int(need), "InceptionV3")
+            if self._ws is None or self._ws.device != dev or self._ws.numel() < need:
+                self._ws = None
+                self._ws = torch.empty(int(need), dtype=torch.uint8, device=dev)
+            outs = (C.c_void_p * 4)()
+            res = []
+            feats = None
+            if pooled:
+                feats = torch.empty(N, _BLOCK_CHANNELS[last], dtype=torch.float32, device=dev)
+            else:
+                for b in self.output_blocks:
+                    h, w = _block_hw(H, W, self.resize_input, b)
+                    res.append(torch.empty(N, _BLOCK_CHANNELS[b], h, w, dtype=torch.float32, device=dev))
+                    outs[b] = res[-1].data_ptr()
+            _lib.check(L.ddpm_inception_forward(self._packed.data_ptr(), x.data_ptr(), N, H, W, int(self.resize_input),
+                                                int(self.normalize_input), last, C.byref(outs),
+                                                None if feats is None else feats.data_ptr(), self._ws.data_ptr(), self._ws.numel(),
+                                                _lib.stream_ptr(dev)), "InceptionV3")
+        return feats if pooled else res
 
     def forward(self, inp):
+        if self.native_eligible(inp):
+            return self.forward_native(inp)
         x = inp
         if self.resize_input:
             x = F.interpolate(x, size=(299, 299), mode="bilinear", align_corners=False)
@@ -120,6 +229,27 @@ class InceptionV3(nn.Module):
             if i in self.output_blocks:
                 out.append(x)
         return out
+
+
+_ENGINE_BLOCK = {"Conv2d_1a_3x3": "blocks.0.0", "Conv2d_2a_3x3": "blocks.0.1", "Conv2d_2b_3x3": "blocks.0.2",
+                 "Conv2d_3b_1x1": "blocks.1.0", "Conv2d_4a_3x3": "blocks.1.1",
+                 **{f"Mixed_{m}": f"blocks.2.{i}" for i, m in enumerate(("5b", "5c", "5d", "6a", "6b", "6c", "6d", "6e"))},
+                 **{f"Mixed_{m}": f"blocks.3.{i}" for i, m in enumerate(("7a", "7b", "7c"))}}
+_BLOCK_CHANNELS = (64, 192, 768, 2048)
+
+
+def _block_hw(H, W, resize, block):
+    """Spatial size of block ``block``'s output for an H x W input."""
+    def one(n):
+        n = 299 if resize else n
+        n = (n - 3) // 2 + 1 - 2                  # Conv2d_1a (3x3 s2), Conv2d_2a (3x3); Conv2d_2b keeps the size
+        n = (n - 3) // 2 + 1                      # max pool: block 0
+        if block >= 1:
+            n = (n - 2 - 3) // 2 + 1              # Conv2d_4a (3x3), max pool: block 1
+        if block >= 2:
+            n = (n - 3) // 2 + 1                  # Mixed_6a: block 2
+        return 1 if block == 3 else n
+    return one(H), one(W)
 
 
 def seeded_state_dict(seed=0):

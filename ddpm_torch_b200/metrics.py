@@ -281,6 +281,9 @@ def calc_pr(manifold_1: Manifold, manifold_2: Manifold, row_batch_size: int, col
 #   with ``ddpm_fid_stats_update`` (a DMMA GEMM, csrc/fid.cuh) on that device's current stream; calc_fd runs ``ddpm_fid_distance``
 #   (two one-sided Jacobi eigen-solves and two DMMA GEMMs), with no scipy.linalg.sqrtm.  Only the final statistics and the distance
 #   come back to the host.
+# * Inception itself runs on the engine whenever ``InceptionV3.native_eligible`` holds (one sm_90 device, eval mode, no gradient;
+#   csrc/inception.cuh), and InceptionStatistics then folds the engine's [N, D] global averages in directly.  A device list keeps
+#   DataParallel over the torch modules, as upstream.
 # * CPU ``device``: the reference's numpy formulas.
 # Three upstream bugs are fixed, each next to its code: sqrtm's removed ``disp`` keyword (calculate_frechet_distance), numpy
 # features handed to adaptive_avg_pool2d for activation_dim != 2048 (InceptionStatistics.forward), and the empty last batch of
@@ -325,6 +328,7 @@ class InceptionStatistics(nn.Module):
         model.requires_grad_(False)
         extractor = _FirstOutput(model)
         if isinstance(self.device, (list, tuple)):
+            model.use_engine = False                           # under DataParallel, on torch, as upstream
             model.to(self.device[0])
             return nn.DataParallel(extractor, device_ids=list(self.device))
         return extractor.to(self.device)
@@ -332,6 +336,11 @@ class InceptionStatistics(nn.Module):
     def forward(self, x):
         x = self.input_transform(x)
         with torch.inference_mode():
+            net = self.model._module if isinstance(self.model, _FirstOutput) else None
+            if self._dev is not None and net is not None and net.native_eligible(x):
+                # the engine's global average of the last block, [N, D] rows fed to the statistics as they are
+                self._fold(net.forward_native(x, pooled=True))
+                return
             act = self.model(x)
             # Upstream pools after .cpu().numpy(), and adaptive_avg_pool2d refuses a numpy array: activation_dim 64 / 192 / 768
             # raised TypeError.  Pooled here, on the features' own device, before they leave it.
@@ -342,11 +351,7 @@ class InceptionStatistics(nn.Module):
         if n == 0:
             return
         if self._dev is not None:
-            feats = act.to(device=self._dev, dtype=torch.float32).contiguous()
-            with torch.cuda.device(self._dev):
-                _lib.check(_lib.lib().ddpm_fid_stats_update(self._state.data_ptr(), self.activation_dim, feats.data_ptr(), n,
-                                                            feats.stride(0), _lib.stream_ptr(self._dev)), "InceptionStatistics")
-            self.count += n
+            self._fold(act)
             return
         act = act.cpu().numpy()
         mean = np.mean(act, axis=0, dtype=np.float64)
@@ -360,6 +365,14 @@ class InceptionStatistics(nn.Module):
             self._mean += alpha * diff
             self._var += alpha * (var - self._var)
             self._var += alpha * (1 - alpha) * np.outer(diff, diff)
+        self.count += n
+
+    def _fold(self, act):
+        n = act.shape[0]
+        feats = act.to(device=self._dev, dtype=torch.float32).contiguous()
+        with torch.cuda.device(self._dev):
+            _lib.check(_lib.lib().ddpm_fid_stats_update(self._state.data_ptr(), self.activation_dim, feats.data_ptr(), n,
+                                                        feats.stride(0), _lib.stream_ptr(self._dev)), "InceptionStatistics")
         self.count += n
 
     def _native_stats(self, ddof):

@@ -223,6 +223,54 @@ int ddpm_fid_distance(const double* mu1, const double* sigma1, const double* mu2
                       void* scratch, long long bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * FID Inception-v3 forward (ddpm_torch/metrics/inception.py; inception.cuh): the 94 BasicConv2d layers (conv, eval BatchNorm
+ * eps = 1e-3, ReLU) as TF32 implicit GEMMs on the tensor cores, the pools and the global average as SIMT kernels, NHWC fp32 inside.
+ * Stateless: every buffer is the caller's, nothing is allocated, nothing synchronises, every call can be captured in a graph, and
+ * every argument is checked before the first launch.  An image's outputs are bit-identical whatever batch it arrives in.
+ * ddpm_inception_num_params / _param_info: the raw parameters in torchvision Inception3's state_dict key order (num_batches_tracked
+ *                         and fc.* left out): 5 per conv (conv.weight [Cout][Cin][kh][kw], bn.weight, bn.bias, bn.running_mean,
+ *                         bn.running_var [Cout]) at fp32 element `offset` of one flat raw buffer.  dims past ndim are 0.
+ * ddpm_inception_conv_info conv i (state_dict order) as the forward runs it: {Cin, Cout, kh, kw, stride, ph, pw, c_off, C_total,
+ *                         1 if it writes the trunk (a stem tensor, or its channel slice of a block output) else 0, its position in
+ *                         the forward's launch order (-1 if the walk did not visit all 94 convs)}.
+ * ddpm_inception_pack     raw (device fp32, 4-byte aligned) -> packed (ddpm_inception_packed_bytes, 256-byte aligned): BatchNorm
+ *                         folded into each conv in fp64 (w gamma / sqrt(var + eps), beta - mean gamma / sqrt(var + eps)), rounded
+ *                         once to fp32; the weights are then rounded to TF32.
+ * ddpm_inception_forward  x NCHW fp32 [N][3][H][W] (device, 4-byte aligned); resize: bilinear to 299 x 299 first (align_corners
+ *                         False); normalize: 2x - 1.  Blocks 0..last_block run; outs[b] (may be null) <- block b NCHW fp32: [N][64][.][.],
+ *                         [N][192][.][.], [N][768][.][.], [N][2048][1][1].  pooled (may be null) <- [N][C] global average of block
+ *                         last_block (for block 3 the same values as outs[3]).  ws: ddpm_inception_workspace_bytes(N, H, W,
+ *                         resize, last_block) bytes, 256-byte aligned; that call refuses (< 0) an input too small for the block.
+ * ddpm_inception_conv_run one conv of the network's kind: x NHWC fp32 [N][H][W][Cin rounded up to 4] (16-byte aligned), raw
+ *                         weights and BatchNorm vectors as in the state_dict, out channels [c_off, c_off + Cout) of NHWC
+ *                         [N][Ho][Wo][C_total] (Cout, c_off, C_total even); scratch: ddpm_inception_conv_scratch_bytes(d).
+ * ddpm_inception_pool_run kind 0: 3 x 3 max, stride 2, no padding; 1: 3 x 3 average, stride 1, padding 1, padding not counted;
+ *                         2: 3 x 3 max, stride 1, padding 1.  x NHWC [N][H][W][C]; out channels [c_off, c_off + C) of [N][Ho][Wo][C_total].
+ * ddpm_inception_input_run the forward's first kernel: x NCHW [N][3][H][W] -> NHWC [N][Ho][Wo][12], Ho = Wo = 299 with resize,
+ *                         else H, W: per pixel {x_hi[3], 0, x_lo[3], 0, x_hi[3], 0}, x_hi = x rounded to TF32, x_lo = x - x_hi, which
+ *                         the first conv's packed weights {w_hi, w_hi, w_lo} turn into a 3xTF32 product. */
+typedef struct {
+    int N, H, W, Cin, Cout, kh, kw, stride, ph, pw, c_off, C_total;
+    const float* x;
+    const float *w, *gamma, *beta, *mean, *var;
+    float* out;
+    void* scratch;
+    long long scratch_bytes;
+} ddpm_inception_conv_desc;
+int ddpm_inception_num_params(void);
+int ddpm_inception_param_info(int i, const char** name, int* ndim, int dims[4], long long* offset);
+int ddpm_inception_conv_info(int i, int info[11]);
+long long ddpm_inception_packed_bytes(void);
+int ddpm_inception_pack(const float* raw, void* packed, void* stream);
+long long ddpm_inception_workspace_bytes(int N, int H, int W, int resize, int last_block);
+int ddpm_inception_forward(const void* packed, const float* x, int N, int H, int W, int resize, int normalize, int last_block,
+                           float* const outs[4], float* pooled, void* ws, long long ws_bytes, void* stream);
+long long ddpm_inception_conv_scratch_bytes(const ddpm_inception_conv_desc* d);
+int ddpm_inception_conv_run(const ddpm_inception_conv_desc* d, void* stream);
+int ddpm_inception_pool_run(int kind, const float* x, int N, int H, int W, int C, float* out, int c_off, int C_total, void* stream);
+int ddpm_inception_input_run(const float* x, int N, int H, int W, int resize, int normalize, float* out, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Low-level operators: GroupNorm(32, C, eps=1e-6) [+ SiLU] [+ dropout] (unet.py:18-20,83-84) and the bias column sums, with the
  * launch geometry the UNet engine's plans use (used by the parity tests of the engine itself).
  * Input = channel concat of two NHWC bf16 sources x0 [B][HW][C0] and x1 [B][HW][C1] (C1 = 0: one source).  C0 and C1 are
