@@ -214,6 +214,12 @@ def lib():
             "ddpm_inception_conv_run": ([C.POINTER(IncConvDesc), vp], i32),
             "ddpm_inception_pool_run": ([i32, vp, i32, i32, i32, i32, vp, i32, i32, vp], i32),
             "ddpm_inception_input_run": ([vp, i32, i32, i32, i32, i32, vp, vp], i32),
+            "ddpm_is_fc_packed_bytes": ([], i64),
+            "ddpm_is_fc_pack": ([vp, vp, vp], i32),
+            "ddpm_is_logits_workspace_bytes": ([i32], i64),
+            "ddpm_is_logits": ([vp, vp, i32, i64, vp, vp, i64, vp], i32),
+            "ddpm_is_score_scratch_bytes": ([i32, i32, i32], i64),
+            "ddpm_is_score": ([vp, i32, i32, i64, i32, vp, vp, i64, vp], i32),
             "ddpm_toy_num_params": ([vp], i64),
             "ddpm_toy_workspace_bytes": ([vp, i64, i32], i64),
             "ddpm_toy_forward": ([vp, vp, vp, vp, i64, vp, i32, vp, i64, vp], i32),
@@ -247,7 +253,9 @@ EXPORTS = ["ddpm_last_error", "ddpm_runtime_check", "ddpm_device_error_flag", "d
            "ddpm_toy_backward", "ddpm_toy_train_backward", "ddpm_toy_sample",
            "ddpm_inception_num_params", "ddpm_inception_param_info", "ddpm_inception_conv_info", "ddpm_inception_packed_bytes", "ddpm_inception_pack",
            "ddpm_inception_workspace_bytes", "ddpm_inception_forward", "ddpm_inception_conv_scratch_bytes", "ddpm_inception_conv_run",
-           "ddpm_inception_pool_run", "ddpm_inception_input_run"]
+           "ddpm_inception_pool_run", "ddpm_inception_input_run",
+           "ddpm_is_fc_packed_bytes", "ddpm_is_fc_pack", "ddpm_is_logits_workspace_bytes", "ddpm_is_logits",
+           "ddpm_is_score_scratch_bytes", "ddpm_is_score"]
 
 
 def check(rc, what=""):

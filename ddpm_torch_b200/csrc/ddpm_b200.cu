@@ -9,6 +9,7 @@
 #include "knn.cuh"
 #include "fid.cuh"
 #include "inception.cuh"
+#include "inception_score.cuh"
 #include "toy_mlp.cuh"
 
 using namespace ddpm;
@@ -711,6 +712,66 @@ int ddpm_inception_input_run(const float* x, int N, int H, int W, int resize, in
     if (normalize != 0 && normalize != 1) return fail(-47, "%s: normalize must be 0 or 1 (got %d)", fn, normalize);
     if (!x || !out || misaligned(x, 4) || misaligned(out, 16)) return fail(-47, "%s: null or misaligned buffer", fn);
     const cudaError_t e = inc_input_launch(x, N, H, W, resize, normalize, out, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? 0 : fail(-20, "%s: launch failed: %s", fn, cudaGetErrorString(e));
+}
+
+// ------------------------------------------------------------------------------------------------ Inception Score
+long long ddpm_is_fc_packed_bytes(void) { return (long long)is_packed_bytes(); }
+
+int ddpm_is_fc_pack(const float* fc_weight, void* packed, void* stream) {
+    const char* fn = "ddpm_is_fc_pack";
+    if (!fc_weight || misaligned(fc_weight, 4)) return fail(-48, "%s: fc_weight must be a non-null, 4-byte aligned fp32 buffer", fn);
+    if (!packed || misaligned(packed, 256)) return fail(-48, "%s: packed must be a non-null, 256-byte aligned buffer", fn);
+    const cudaError_t e = is_pack_launch(fc_weight, static_cast<float*>(packed), static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? 0 : fail(-20, "%s: launch failed: %s", fn, cudaGetErrorString(e));
+}
+
+static int is_check_n(const char* fn, int N) {
+    if (N < 1) return fail(-48, "%s: N must be >= 1 (got %d)", fn, N);
+    return 0;
+}
+
+long long ddpm_is_logits_workspace_bytes(int N) {
+    if (int rc = is_check_n("ddpm_is_logits_workspace_bytes", N)) return rc;
+    return (long long)is_logits_ws_bytes(N);
+}
+
+int ddpm_is_logits(const void* packed, const float* feats, int N, long long ld, float* logits, void* ws, long long ws_bytes, void* stream) {
+    const char* fn = "ddpm_is_logits";
+    if (int rc = is_check_n(fn, N)) return rc;
+    if (!packed || misaligned(packed, 256)) return fail(-48, "%s: packed must be a non-null, 256-byte aligned buffer", fn);
+    if (!feats || misaligned(feats, 4)) return fail(-48, "%s: feats must be a non-null, 4-byte aligned fp32 buffer", fn);
+    if (ld < IS_FEAT) return fail(-48, "%s: row pitch ld = %lld must be >= %d", fn, ld, IS_FEAT);
+    if (!logits || misaligned(logits, 8)) return fail(-48, "%s: logits must be a non-null, 8-byte aligned fp32 buffer", fn);
+    const size_t need = is_logits_ws_bytes(N);
+    if (!ws || misaligned(ws, 256) || ws_bytes < (long long)need)
+        return fail(-48, "%s: needs a 256-byte aligned workspace of ddpm_is_logits_workspace_bytes = %zu bytes (got %lld)", fn, need, ws_bytes);
+    const cudaError_t e = is_logits_launch(static_cast<const float*>(packed), feats, ld, N, logits, ws, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? 0 : fail(-20, "%s: launch failed: %s", fn, cudaGetErrorString(e));
+}
+
+static int is_check_score(const char* fn, int N, int C, int splits) {
+    if (C < 1) return fail(-48, "%s: C must be >= 1 (got %d)", fn, C);
+    if (splits < 1 || splits > N) return fail(-48, "%s: needs 1 <= splits <= N (N = %d, splits = %d)", fn, N, splits);
+    if ((long long)splits * is_chunks(N, splits) * is_col_blocks(C) > INT_MAX) return fail(-48, "%s: splits * C too large", fn);
+    return 0;
+}
+
+long long ddpm_is_score_scratch_bytes(int N, int C, int splits) {
+    if (int rc = is_check_score("ddpm_is_score_scratch_bytes", N, C, splits)) return rc;
+    return (long long)is_score_bytes(N, C, splits);
+}
+
+int ddpm_is_score(const float* logits, int N, int C, long long ld, int splits, double* out, void* scratch, long long bytes, void* stream) {
+    const char* fn = "ddpm_is_score";
+    if (int rc = is_check_score(fn, N, C, splits)) return rc;
+    if (!logits || misaligned(logits, 4)) return fail(-48, "%s: logits must be a non-null, 4-byte aligned fp32 buffer", fn);
+    if (ld < C) return fail(-48, "%s: row pitch ld = %lld must be >= C = %d", fn, ld, C);
+    if (!out || misaligned(out, 8)) return fail(-48, "%s: out must be a non-null, 8-byte aligned fp64 buffer of splits + 1 values", fn);
+    const size_t need = is_score_bytes(N, C, splits);
+    if (!scratch || misaligned16(scratch) || bytes < (long long)need)
+        return fail(-48, "%s: needs a 16-byte aligned scratch of ddpm_is_score_scratch_bytes = %zu bytes (got %lld)", fn, need, bytes);
+    const cudaError_t e = is_score_launch(logits, ld, N, C, splits, out, scratch, static_cast<cudaStream_t>(stream));
     return e == cudaSuccess ? 0 : fail(-20, "%s: launch failed: %s", fn, cudaGetErrorString(e));
 }
 

@@ -82,8 +82,10 @@ __host__ __device__ constexpr int inc_smem_bytes() { return INC_STAGES * inc_sta
 // Chunk c (16 bytes) of row r of a 128-byte-swizzled K-major tile lives at r * 128 + ((c ^ (r & 7)) << 4).
 __device__ __forceinline__ uint32_t inc_swz(int r, int c) { return (uint32_t)(r * 128 + ((c ^ (r & 7)) << 4)); }
 
-template <int BN>
-__global__ void __launch_bounds__(INC_THREADS, 1) inc_conv_tf32_kernel(const IncConvArgs a) {
+// The GEMM body shared by the convolutions and the Inception Score's logits (inception_score.cuh).  BN_RELU: the convolutions'
+// epilogue (folded BatchNorm bias, then ReLU); without it the raw fp32 accumulators are stored.
+template <int BN, bool BN_RELU>
+__device__ __forceinline__ void inc_conv_tf32_body(const IncConvArgs& a) {
     extern __shared__ uint8_t inc_smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(inc_smem_raw) + 1023) & ~uintptr_t(1023));
     constexpr int STAGE = inc_stage_bytes<BN>();
@@ -176,13 +178,19 @@ __global__ void __launch_bounds__(INC_THREADS, 1) inc_conv_tf32_kernel(const Inc
         for (int j = 0; j < BN / 8; ++j) {
             const int col = n0 + 8 * j + 2 * (l & 3);
             if (col < a.Cout) {                                  // Cout is even: col + 1 < Cout too
-                float v0 = acc[4 * j + 2 * h] + __ldg(a.bias + col), v1 = acc[4 * j + 2 * h + 1] + __ldg(a.bias + col + 1);
-                v0 = v0 < 0.f ? 0.f : v0; v1 = v1 < 0.f ? 0.f : v1;
+                float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+                if constexpr (BN_RELU) {
+                    v0 += __ldg(a.bias + col); v1 += __ldg(a.bias + col + 1);
+                    v0 = v0 < 0.f ? 0.f : v0; v1 = v1 < 0.f ? 0.f : v1;
+                }
                 *reinterpret_cast<float2*>(orow + col) = make_float2(v0, v1);
             }
         }
     }
 }
+
+template <int BN>
+__global__ void __launch_bounds__(INC_THREADS, 1) inc_conv_tf32_kernel(const IncConvArgs a) { inc_conv_tf32_body<BN, true>(a); }
 
 // BatchNorm folded into the conv, in fp64, rounded once to fp32 and then to TF32 (the value the tensor core multiplies):
 // w' = w gamma / sqrt(var + eps) laid out [Cout_pad][Kp] with k = (ky kw + kx) Cin4 + ci, zero outside the layer;

@@ -4,7 +4,7 @@ engine (``ddpm_inception_forward``: TF32 tensor-core convolutions with BatchNorm
 else (CPU, autograd, training-mode BatchNorm, ``DataParallel`` replicas, other dtypes) runs the torch modules below.
 
 The FID network differs from torchvision's ImageNet Inception-v3 in three places, all reproduced here:
-  * 1008 classes (its ``fc`` is part of the checkpoint, though no feature uses it);
+  * 1008 classes (its ``fc`` is part of the checkpoint; only the Inception Score uses it, as ``InceptionV3.fc_weight``);
   * the 3x3 average pools inside the A, C and E blocks exclude the padding (TensorFlow's ``count_include_pad=False``);
   * the last E block (``Mixed_7c``) pools its pool branch with a 3x3 max pool.
 Module names follow torchvision's ``Inception3``, so the published ``pt_inception-2015-12-05-6726825d.pth`` loads with
@@ -112,6 +112,9 @@ class InceptionV3(nn.Module):
             [net.Mixed_7a, net.Mixed_7b, net.Mixed_7c, nn.AdaptiveAvgPool2d(output_size=(1, 1))],
         ]
         self.blocks = nn.ModuleList(nn.Sequential(*s) for s in stages[:self.last_needed_block + 1])
+        # the checkpoint's 1008-way fc weight [1008, 2048] (the Inception Score's logits, metrics.InceptionScore): a plain CPU
+        # tensor, so it is neither in the state_dict nor moved or replicated with the module
+        self.fc_weight = net.fc.weight.detach()
         self.requires_grad_(requires_grad)
         self.use_engine = True             # False: always the torch modules (InceptionStatistics over a device list)
         self._native_tensors = None        # the engine's raw parameters, in its order (None: not gathered yet)

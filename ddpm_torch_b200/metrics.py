@@ -1,6 +1,7 @@
 """The evaluation metrics of ``ddpm_torch/metrics``: improved precision and recall (Kynkäänniemi et al., 2019) of
-``precision_recall.py`` with its k-NN half on the engine, and FID (``fid_score.py``, ``__init__.py``'s ``Evaluator``) with its
-statistics and Fréchet distance on the engine (see the FID section below).
+``precision_recall.py`` with its k-NN half on the engine, FID (``fid_score.py``, ``__init__.py``'s ``Evaluator``) with its
+statistics and Fréchet distance on the engine (see the FID section below), and the Inception Score (``InceptionScore``, ``calc_is``;
+see its section), which the reference does not have.
 
 Public names, signatures and defaults are the reference's: ``Manifold``, ``ManifoldBuilder``, ``calc_pr``,
 ``compute_distance``, ``to_uint8`` and ``VGGFeatureExtractor``.
@@ -589,5 +590,185 @@ class Evaluator:
         return {"fid": fid}
 
 
+# ================================================================================================ Inception Score
+# Salimans et al. (2016) as the TensorFlow improved-gan/inception_score.py computes it, which is what papers report: p = softmax over
+# all 1008 classes of pool3 . W^T (W the checkpoint's fc.weight, no bias), the N images cut in order into ``splits`` parts, part i
+# being rows [i N // splits, (i + 1) N // splits), IS_i = exp(mean_x sum_y p(y|x) (log p(y|x) - log pbar_i(y))), and the mean and
+# population std of the IS_i.
+# * CUDA ``device``: the logits are a 3xTF32 GEMM (``ddpm_is_logits``, csrc/inception_score.cuh) that stays on the device, and the
+#   score is ``ddpm_is_score`` in fp64 with fixed-order reductions, so it is bit-identical however the images were batched.
+#   Inception runs on the engine when ``InceptionV3.native_eligible`` holds; a device list runs DataParallel over the torch modules,
+#   then the logits and the score on the first device.
+# * CPU ``device``: the torch modules, fp32 ``x @ W.T`` and the same formula in numpy fp64.
+# Both take log p as z - logsumexp(z) in fp64, where the TF code takes np.log of an fp32 softmax: on well-conditioned logits the two
+# agree to rounding, and a saturated row (a p that underflows in fp32) stays finite here.
+
+IS_CLASSES = 1008
+IS_FEATURES = 2048
+IS_STATUS = {1: "a non-finite logit"}
+
+
+def _is_pack(fc_weight, dev):
+    """fc.weight [1008, 2048] packed on ``dev`` for ``_is_logits`` (``ddpm_is_fc_pack``)."""
+    L = _lib.lib()
+    with torch.cuda.device(dev):
+        w = torch.as_tensor(fc_weight).to(device=dev, dtype=torch.float32).contiguous()
+        if tuple(w.shape) != (IS_CLASSES, IS_FEATURES):
+            raise ValueError(f"fc weight must be [{IS_CLASSES}, {IS_FEATURES}], got {tuple(w.shape)}")
+        packed = torch.empty(L.ddpm_is_fc_packed_bytes(), dtype=torch.uint8, device=dev)
+        _lib.check(L.ddpm_is_fc_pack(w.data_ptr(), packed.data_ptr(), _lib.stream_ptr(dev)), "InceptionScore")
+    return packed
+
+
+def _is_logits(packed, feats, dev, ws=None):
+    """fp32 [N, 1008] logits on ``dev`` of [N, 2048] features (``ddpm_is_logits``).  ``ws``: a uint8 workspace to reuse when it is
+    large enough.  Returns ``(logits, ws)``."""
+    L = _lib.lib()
+    with torch.cuda.device(dev):
+        f = feats.to(device=dev, dtype=torch.float32)
+        if f.dim() != 2 or f.shape[1] != IS_FEATURES:
+            raise ValueError(f"features must be [N, {IS_FEATURES}], got {tuple(f.shape)}")
+        if f.stride(1) != 1 or f.stride(0) < IS_FEATURES:
+            f = f.contiguous()
+        n = f.shape[0]
+        need = L.ddpm_is_logits_workspace_bytes(n)
+        if need < 0:
+            _lib.check(int(need), "is_logits_workspace_bytes")
+        if ws is None or ws.device != dev or ws.numel() < need:
+            ws = None
+            ws = torch.empty(need, dtype=torch.uint8, device=dev)
+        out = torch.empty(n, IS_CLASSES, dtype=torch.float32, device=dev)
+        _lib.check(L.ddpm_is_logits(packed.data_ptr(), f.data_ptr(), n, f.stride(0), out.data_ptr(), ws.data_ptr(), ws.numel(),
+                                    _lib.stream_ptr(dev)), "InceptionScore")
+    return out, ws
+
+
+def _is_check(n, splits):
+    if splits < 1 or n < splits:
+        raise ValueError(f"the Inception Score needs 1 <= splits <= N (N = {n}, splits = {splits})")
+
+
+def _is_numpy(logits, splits):
+    z = np.asarray(logits, dtype=np.float64)
+    if not np.isfinite(z).all():
+        raise ValueError(f"calc_is: {IS_STATUS[1]}")
+    m = z.max(axis=1, keepdims=True)
+    logp = z - (m + np.log(np.exp(z - m).sum(axis=1, keepdims=True)))
+    p = np.exp(logp)
+    n = z.shape[0]
+    scores = []
+    for i in range(splits):
+        b, e = i * n // splits, (i + 1) * n // splits
+        pbar = p[b:e].mean(axis=0)
+        nz = pbar > 0                                     # 0 log 0 = 0
+        kl = np.sum(p[b:e] * logp[b:e]) / (e - b) - np.sum(pbar[nz] * np.log(pbar[nz]))
+        scores.append(np.exp(kl))
+    return scores
+
+
+def _is_native(logits, splits, dev):
+    L = _lib.lib()
+    with torch.cuda.device(dev):
+        z = torch.as_tensor(logits).to(device=dev, dtype=torch.float32)
+        if z.stride(1) != 1 or z.stride(0) < z.shape[1]:
+            z = z.contiguous()
+        n, c = z.shape
+        nbytes = L.ddpm_is_score_scratch_bytes(n, c, splits)
+        if nbytes < 0:
+            _lib.check(int(nbytes), "is_score_scratch_bytes")
+        scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        out = torch.empty(splits + 1, dtype=torch.float64, device=dev)
+        _lib.check(L.ddpm_is_score(z.data_ptr(), n, c, z.stride(0), splits, out.data_ptr(), scratch.data_ptr(), nbytes,
+                                   _lib.stream_ptr(dev)), "calc_is")
+        o = out.cpu().numpy()
+    status = int(o[splits])
+    if status:
+        raise ValueError(f"calc_is: {IS_STATUS[status]}")
+    return list(o[:splits])
+
+
+def calc_is(logits, splits=10, device=None):
+    """Inception Score ``(mean, std)`` (Python floats) of [N, C] logits (a tensor or an array; C = 1008 for the Inception network),
+    cut in order into ``splits`` parts.  On the device of a CUDA tensor, on a CUDA ``device``, or else on the current CUDA device
+    when one is present: ``ddpm_is_score``.  Otherwise (a CPU ``device``, or no CUDA device): the same formula in numpy fp64.
+    ValueError for N < splits or a non-finite logit."""
+    shape = tuple(logits.shape)
+    if len(shape) != 2 or shape[1] < 1:
+        raise ValueError(f"logits must be [N, C], got {shape}")
+    _is_check(shape[0], splits)
+    dev = _fd_device((logits,), device)
+    if dev is None:
+        z = logits.detach().cpu().numpy() if isinstance(logits, torch.Tensor) else logits
+        scores = _is_numpy(z, splits)
+    else:
+        scores = _is_native(logits, splits, dev)
+    return float(np.mean(scores)), float(np.std(scores))
+
+
+class InceptionScore(nn.Module):
+    """Inception Score of every batch passed to ``forward`` (see the section comment above), shaped like InceptionStatistics.
+
+    ``forward(x)`` takes images in [-1, 1] after ``input_transform``, of any size (resized to 299 x 299 as for FID), and keeps their
+    1008-way logits: on a CUDA ``device`` (or the first device of a list, where Inception runs under ``DataParallel``) fp32 on that
+    device, 4 KB per image; on the CPU in host memory.  ``get_score()`` returns ``(mean, std)`` as Python floats; ``reset()`` drops
+    the logits.  The fc weights are the checkpoint's (``weights_path()``), read with the network."""
+
+    def __init__(self, splits=10, input_transform=lambda x: x, device=torch.device("cpu")):
+        super().__init__()
+        self.splits = splits
+        self.input_transform = input_transform
+        self.device = device
+        self.model = self.load_model()
+        self._dev = _cuda_device(_op_device(device))
+        net = self.model.module._module if isinstance(self.model, nn.DataParallel) else self.model._module
+        if self._dev is not None:
+            self._packed = _is_pack(net.fc_weight, self._dev)
+        else:
+            self._fc = net.fc_weight.to(torch.float32)
+        self._ws = None
+        self._logits = []
+        self.count = 0
+
+    def load_model(self):
+        model = InceptionV3([3])
+        model.eval()
+        model.requires_grad_(False)
+        extractor = _FirstOutput(model)
+        if isinstance(self.device, (list, tuple)):
+            model.use_engine = False                           # under DataParallel, on torch, as InceptionStatistics
+            model.to(self.device[0])
+            return nn.DataParallel(extractor, device_ids=list(self.device))
+        return extractor.to(self.device)
+
+    def forward(self, x):
+        x = self.input_transform(x)
+        with torch.inference_mode():
+            net = self.model._module if isinstance(self.model, _FirstOutput) else None
+            if self._dev is not None and net is not None and net.native_eligible(x):
+                feats = net.forward_native(x, pooled=True)
+            else:
+                feats = self.model(x).flatten(1)
+            n = feats.shape[0]
+            if n == 0:
+                return
+            if self._dev is not None:
+                logits, self._ws = _is_logits(self._packed, feats, self._dev, self._ws)
+            else:
+                logits = feats.to(device="cpu", dtype=torch.float32) @ self._fc.T
+            self._logits.append(logits)
+        self.count += n
+
+    def get_score(self):
+        _is_check(self.count, self.splits)
+        if len(self._logits) > 1:
+            self._logits = [torch.cat(self._logits)]
+        return calc_is(self._logits[0], self.splits, device=self._dev if self._dev is not None else "cpu")
+
+    def reset(self):
+        self._logits = []
+        self.count = 0
+
+
 __all__ = ["Manifold", "ManifoldBuilder", "calc_pr", "compute_distance", "to_uint8", "VGGFeatureExtractor",
-           "InceptionV3", "InceptionStatistics", "get_precomputed", "calc_fd", "calculate_frechet_distance", "Evaluator"]
+           "InceptionV3", "InceptionStatistics", "get_precomputed", "calc_fd", "calculate_frechet_distance", "Evaluator",
+           "InceptionScore", "calc_is"]

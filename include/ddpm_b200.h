@@ -271,6 +271,29 @@ int ddpm_inception_pool_run(int kind, const float* x, int N, int H, int W, int C
 int ddpm_inception_input_run(const float* x, int N, int H, int W, int resize, int normalize, float* out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Inception Score (Salimans et al., 2016, as the TensorFlow improved-gan/inception_score.py computes it; inception_score.cuh).
+ * Stateless and graph-capturable like the forward; every argument is checked before the first launch.
+ * ddpm_is_fc_pack         fc_weight (device fp32 [1008][2048], the checkpoint's fc.weight, 4-byte aligned) -> packed
+ *                         (ddpm_is_fc_packed_bytes, 256-byte aligned): per class [w_hi | w_hi | w_lo] with w_hi = tf32(w),
+ *                         w_lo = tf32(w - w_hi).
+ * ddpm_is_logits          logits fp32 [N][1008] (row pitch 1008, 8-byte aligned) = feats . fc_weight^T, no bias; feats fp32 [N]
+ *                         rows of pitch ld >= 2048 (the pooled block-3 features).  A 3xTF32 GEMM (f_hi w_hi + f_lo w_hi + f_hi w_lo,
+ *                         fp32 accumulation); a row depends on its own features only.  ws: ddpm_is_logits_workspace_bytes(N)
+ *                         bytes, 256-byte aligned.
+ * ddpm_is_score           logits fp32 [N][C] (row pitch ld >= C), cut in order into `splits` parts, part i = rows
+ *                         [i N / splits, (i + 1) N / splits), 1 <= splits <= N.  out (fp64, splits + 1 values): out[i] =
+ *                         exp(mean_x sum_y p(y|x) (log p(y|x) - log pbar_i(y))) with p = softmax over all C classes, computed in fp64
+ *                         with log p = z - logsumexp(z); out[splits] = status: 0, or 1 when a logit is not finite (then out[i] are
+ *                         NaN).  Fixed-order reductions: the same logits give the same bits.  scratch: ddpm_is_score_scratch_bytes(N,
+ *                         C, splits) bytes, 16-byte aligned. */
+long long ddpm_is_fc_packed_bytes(void);
+int ddpm_is_fc_pack(const float* fc_weight, void* packed, void* stream);
+long long ddpm_is_logits_workspace_bytes(int N);
+int ddpm_is_logits(const void* packed, const float* feats, int N, long long ld, float* logits, void* ws, long long ws_bytes, void* stream);
+long long ddpm_is_score_scratch_bytes(int N, int C, int splits);
+int ddpm_is_score(const float* logits, int N, int C, long long ld, int splits, double* out, void* scratch, long long bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Low-level operators: GroupNorm(32, C, eps=1e-6) [+ SiLU] [+ dropout] (unet.py:18-20,83-84) and the bias column sums, with the
  * launch geometry the UNet engine's plans use (used by the parity tests of the engine itself).
  * Input = channel concat of two NHWC bf16 sources x0 [B][HW][C0] and x1 [B][HW][C1] (C1 = 0: one source).  C0 and C1 are
