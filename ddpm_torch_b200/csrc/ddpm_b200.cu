@@ -10,6 +10,7 @@
 #include "fid.cuh"
 #include "inception.cuh"
 #include "inception_score.cuh"
+#include "kid.cuh"
 #include "toy_mlp.cuh"
 
 using namespace ddpm;
@@ -772,6 +773,50 @@ int ddpm_is_score(const float* logits, int N, int C, long long ld, int splits, d
     if (!scratch || misaligned16(scratch) || bytes < (long long)need)
         return fail(-48, "%s: needs a 16-byte aligned scratch of ddpm_is_score_scratch_bytes = %zu bytes (got %lld)", fn, need, bytes);
     const cudaError_t e = is_score_launch(logits, ld, N, C, splits, out, scratch, static_cast<cudaStream_t>(stream));
+    return e == cudaSuccess ? 0 : fail(-20, "%s: launch failed: %s", fn, cudaGetErrorString(e));
+}
+
+// ------------------------------------------------------------------------------------------------ Kernel Inception Distance
+static int kid_check_sizes(const char* fn, int S, int m) {
+    if (S < 1) return fail(-49, "%s: S (the number of subsets) must be >= 1 (got %d)", fn, S);
+    if (m < 2) return fail(-49, "%s: m (the subset size) must be >= 2 (got %d)", fn, m);
+    if ((long long)S * kid_blocks(m) > INT_MAX || (long long)S * 2 * m > INT_MAX) return fail(-49, "%s: S * m too large", fn);
+    return 0;
+}
+
+long long ddpm_kid_scratch_bytes(int S, int m) {
+    if (int rc = kid_check_sizes("ddpm_kid_scratch_bytes", S, m)) return rc;
+    return (long long)kid_bytes(S, m);
+}
+
+int ddpm_kid(const float* x, long long ldx, int n1, const float* y, long long ldy, int n2, int d, const int32_t* idx_host, int S, int m,
+             int degree, double gamma, double coef0, double* out, void* scratch, long long bytes, void* stream) {
+    const char* fn = "ddpm_kid";
+    if (int rc = kid_check_sizes(fn, S, m)) return rc;
+    if (d < 1 || d > FID_MAX_D) return fail(-49, "%s: d must be in 1..%d (got %d)", fn, FID_MAX_D, d);
+    if (m > n1 || m > n2) return fail(-49, "%s: needs 2 <= m <= min(n1, n2) (m = %d, n1 = %d, n2 = %d)", fn, m, n1, n2);
+    if (!x || misaligned(x, 4) || !y || misaligned(y, 4)) return fail(-49, "%s: x and y must be non-null, 4-byte aligned fp32 buffers", fn);
+    if (ldx < d || ldy < d) return fail(-49, "%s: row pitches ldx = %lld, ldy = %lld must be >= d = %d", fn, ldx, ldy, d);
+    if (degree < 1 || degree > KID_MAX_DEGREE) return fail(-49, "%s: degree must be in 1..%d (got %d)", fn, KID_MAX_DEGREE, degree);
+    if (!idx_host) return fail(-49, "%s: idx_host must be a non-null host array of S * 2 * m indices", fn);
+    if (!out || misaligned(out, 8)) return fail(-49, "%s: out must be a non-null, 8-byte aligned fp64 buffer of S + 3 values", fn);
+    const size_t need = kid_bytes(S, m);
+    if (!scratch || misaligned16(scratch) || bytes < (long long)need)
+        return fail(-49, "%s: needs a 16-byte aligned scratch of ddpm_kid_scratch_bytes = %zu bytes (got %lld)", fn, need, bytes);
+    // every index in range and distinct within its half of a subset, so the kernels never see a bad row
+    std::vector<int> seen((size_t)std::max(n1, n2), -1);
+    for (int h = 0; h < 2 * S; ++h) {
+        const int n = h & 1 ? n2 : n1;
+        const int32_t* ix = idx_host + (size_t)h * m;
+        for (int i = 0; i < m; ++i) {
+            const int v = ix[i];
+            if (v < 0 || v >= n)
+                return fail(-49, "%s: subset %d: index %d of %s is out of range 0..%d", fn, h / 2, v, h & 1 ? "iy" : "ix", n - 1);
+            if (seen[v] == h) return fail(-49, "%s: subset %d: index %d repeats in %s", fn, h / 2, v, h & 1 ? "iy" : "ix");
+            seen[v] = h;
+        }
+    }
+    const cudaError_t e = kid_launch(x, ldx, y, ldy, d, idx_host, S, m, degree, gamma, coef0, out, scratch, static_cast<cudaStream_t>(stream));
     return e == cudaSuccess ? 0 : fail(-20, "%s: launch failed: %s", fn, cudaGetErrorString(e));
 }
 

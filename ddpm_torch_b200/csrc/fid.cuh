@@ -114,6 +114,14 @@ __device__ __forceinline__ void fid_load_chunk(const T* __restrict__ X, long lon
     }
 }
 
+// the t-th tile (ti, tj) of a lower triangle including the diagonal, row by row: t = ti (ti + 1) / 2 + tj, tj <= ti
+__device__ __forceinline__ void fid_tri_tile(int t, int& ti, int& tj) {
+    ti = (int)((sqrt(8.0 * t + 1.0) - 1.0) * 0.5);
+    while (ti * (ti + 1) / 2 > t) --ti;
+    while ((ti + 1) * (ti + 2) / 2 <= t) ++ti;
+    tj = t - ti * (ti + 1) / 2;
+}
+
 template <typename T>
 __global__ void __launch_bounds__(256) k_fid_gemm(FidGemm p) {
     pdl_entry();
@@ -121,11 +129,7 @@ __global__ void __launch_bounds__(256) k_fid_gemm(FidGemm p) {
     __shared__ double xs[FID_KC][FID_SPAD], ys[FID_KC][FID_SPAD];
     int ti, tj;
     if (p.lower) {
-        const int t = blockIdx.x;
-        ti = (int)((sqrt(8.0 * t + 1.0) - 1.0) * 0.5);
-        while (ti * (ti + 1) / 2 > t) --ti;
-        while ((ti + 1) * (ti + 2) / 2 <= t) ++ti;
-        tj = t - ti * (ti + 1) / 2;
+        fid_tri_tile(blockIdx.x, ti, tj);
     } else {
         ti = blockIdx.x / p.tiles; tj = blockIdx.x % p.tiles;
     }

@@ -1,7 +1,7 @@
 """The evaluation metrics of ``ddpm_torch/metrics``: improved precision and recall (Kynkäänniemi et al., 2019) of
 ``precision_recall.py`` with its k-NN half on the engine, FID (``fid_score.py``, ``__init__.py``'s ``Evaluator``) with its
-statistics and Fréchet distance on the engine (see the FID section below), and the Inception Score (``InceptionScore``, ``calc_is``;
-see its section), which the reference does not have.
+statistics and Fréchet distance on the engine (see the FID section below), and the Inception Score (``InceptionScore``, ``calc_is``)
+and the Kernel Inception Distance (``KernelInceptionDistance``, ``calc_kid``; see their sections), which the reference does not have.
 
 Public names, signatures and defaults are the reference's: ``Manifold``, ``ManifoldBuilder``, ``calc_pr``,
 ``compute_distance``, ``to_uint8`` and ``VGGFeatureExtractor``.
@@ -769,6 +769,180 @@ class InceptionScore(nn.Module):
         self.count = 0
 
 
+# ================================================================================================ Kernel Inception Distance
+# Bińkowski et al. (2018), "Demystifying MMD GANs": the unbiased estimator of the squared MMD with the polynomial kernel
+# k(x, y) = (gamma x . y + coef0)^degree (gamma = 1 / d by default), averaged over ``num_subsets`` subsets of ``subset_size`` = m rows
+# of each feature set:
+#   mmd2_s = (sum_{i != j} k(x_i, x_j) + sum_{i != j} k(y_i, y_j)) / (m (m - 1)) - 2 sum_{i, j} k(x_i, y_j) / m^2,
+# and the mean and population std (ddof = 0) of the mmd2_s.  Unlike FID its expectation does not depend on the sample count, so it
+# is the metric to compare runs evaluated on a few thousand samples.  Subset s takes ix = rng.choice(n1, m, replace=False), then
+# iy = rng.choice(n2, m, replace=False), from one ``np.random.RandomState(seed)``; the indices are drawn on the host, so both paths
+# see the same subsets.
+# * CUDA ``device``: ``ddpm_kid`` (csrc/kid.cuh), fp64 Gram tiles on the DMMA tensor cores with the kernel and the sums fused in, no
+#   m x m matrix in memory, every sum in a fixed order: bit-identical from run to run and however the features were batched.
+# * CPU ``device``: the same formula in numpy fp64, the reference the tests compare against.
+
+KID_STATUS = {1: "a non-finite feature or kernel value"}
+KID_MAX_DEGREE = 8                                        # csrc/kid.cuh
+KID_KERNEL_ARGS = ("degree", "gamma", "coef0", "seed")
+
+
+def _kid_indices(n1, n2, num_subsets, subset_size, seed):
+    """int32 [num_subsets, 2, subset_size]: per subset ix (rows of the first set) then iy (rows of the second), drawn in that order."""
+    rng = np.random.RandomState(seed)
+    idx = np.empty((num_subsets, 2, subset_size), dtype=np.int32)
+    for s in range(num_subsets):
+        idx[s, 0] = rng.choice(n1, subset_size, replace=False)
+        idx[s, 1] = rng.choice(n2, subset_size, replace=False)
+    return idx
+
+
+def _kid_numpy(x, y, idx, degree, gamma, coef0):
+    """mmd2_s per subset in numpy fp64 (features cast to fp64 first)."""
+    x = np.asarray(x, dtype=np.float64)
+    y = np.asarray(y, dtype=np.float64)
+    m = idx.shape[2]
+    out = np.empty(idx.shape[0])
+    with np.errstate(invalid="ignore", over="ignore"):          # a non-finite value is reported by the caller
+        for s in range(idx.shape[0]):
+            a, b = x[idx[s, 0]], y[idx[s, 1]]
+            kxx = (gamma * (a @ a.T) + coef0) ** degree
+            kyy = (gamma * (b @ b.T) + coef0) ** degree
+            kxy = (gamma * (a @ b.T) + coef0) ** degree
+            out[s] = (kxx.sum() - np.trace(kxx) + kyy.sum() - np.trace(kyy)) / (m * (m - 1)) - 2 * kxy.sum() / (m * m)
+    return out
+
+
+def _kid_rows(f, dev):
+    f = torch.as_tensor(f).to(device=dev, dtype=torch.float32)
+    return f if f.stride(1) == 1 and f.stride(0) >= f.shape[1] else f.contiguous()
+
+
+def _kid_native(x, y, idx, degree, gamma, coef0, dev):
+    """``ddpm_kid`` on ``dev``'s current stream: the numpy array of mmd2_s per subset and the status."""
+    L = _lib.lib()
+    S, _, m = idx.shape
+    idx = np.ascontiguousarray(idx, dtype=np.int32)
+    with torch.cuda.device(dev):
+        a, b = _kid_rows(x, dev), _kid_rows(y, dev)
+        nbytes = L.ddpm_kid_scratch_bytes(S, m)
+        if nbytes < 0:
+            _lib.check(int(nbytes), "kid_scratch_bytes")
+        scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        out = torch.empty(S + 3, dtype=torch.float64, device=dev)
+        _lib.check(L.ddpm_kid(a.data_ptr(), a.stride(0), a.shape[0], b.data_ptr(), b.stride(0), b.shape[0], a.shape[1],
+                              idx.ctypes.data, S, m, degree, gamma, coef0, out.data_ptr(), scratch.data_ptr(), nbytes,
+                              _lib.stream_ptr(dev)), "calc_kid")
+        o = out.cpu().numpy()
+    return o[:S], int(o[S + 2])
+
+
+def calc_kid(features1, features2, num_subsets=100, subset_size=1000, degree=3, gamma=None, coef0=1., seed=1234, device=None):
+    """Kernel Inception Distance ``(mean, std)`` (Python floats) between [n1, d] and [n2, d] features (tensors or arrays), as defined
+    in the section comment above.  This follows the unbiased estimator as torch-fidelity and clean-fid compute it (subset MMD^2
+    with the cubic polynomial kernel, mean and population std); it has not been checked against either, which are not
+    dependencies of this project.  On the device of a CUDA tensor, on a CUDA ``device``, or else on the current CUDA device when one
+    is present: ``ddpm_kid``.  Otherwise (a CPU ``device``, or no CUDA device): numpy fp64.  ValueError for inputs that are not 2-D,
+    a feature-dimension mismatch or d outside 1..4096, ``subset_size`` outside 2..min(n1, n2), ``num_subsets`` < 1, ``degree``
+    outside 1..8, and a non-finite feature in a drawn row or a non-finite kernel value."""
+    s1, s2 = tuple(features1.shape), tuple(features2.shape)
+    if len(s1) != 2 or len(s2) != 2:
+        raise ValueError(f"features must be [n, d], got {s1} and {s2}")
+    (n1, d), n2 = s1, s2[0]
+    if s2[1] != d:
+        raise ValueError(f"feature dimensions differ: {d} and {s2[1]}")
+    if not 1 <= d <= 4096:
+        raise ValueError(f"the feature dimension must be in 1..4096, got {d}")
+    if not 2 <= subset_size <= min(n1, n2):
+        raise ValueError(f"the KID needs 2 <= subset_size <= min(n1, n2) (subset_size = {subset_size}, n1 = {n1}, n2 = {n2})")
+    if num_subsets < 1:
+        raise ValueError(f"num_subsets must be >= 1, got {num_subsets}")
+    if int(degree) != degree or not 1 <= degree <= KID_MAX_DEGREE:
+        raise ValueError(f"degree must be an integer in 1..{KID_MAX_DEGREE}, got {degree}")
+    degree = int(degree)
+    gamma = 1.0 / d if gamma is None else float(gamma)
+    idx = _kid_indices(n1, n2, num_subsets, subset_size, seed)
+    dev = _fd_device((features1, features2), device)
+    if dev is None:
+        host = [f.detach().cpu().numpy() if isinstance(f, torch.Tensor) else f for f in (features1, features2)]
+        mmd = _kid_numpy(host[0], host[1], idx, degree, gamma, float(coef0))
+        status = 0 if np.isfinite(mmd).all() else 1
+    else:
+        mmd, status = _kid_native(features1, features2, idx, degree, gamma, float(coef0), dev)
+    if status:
+        raise ValueError(f"calc_kid: {KID_STATUS[status]}")
+    return float(np.mean(mmd)), float(np.std(mmd))
+
+
+class KernelInceptionDistance(nn.Module):
+    """Kernel Inception Distance of every batch passed to ``forward`` against another feature set (see the section comment above),
+    shaped like InceptionScore.
+
+    ``forward(x)`` takes images in [-1, 1] after ``input_transform``, of any size (resized to 299 x 299 as for FID), and keeps their
+    2048 pool3 features: on a CUDA ``device`` (or the first device of a list, where Inception runs under ``DataParallel``) fp32 on
+    that device, 8 KB per image; on the CPU in host memory.  ``features`` is the [N, 2048] tensor of all of them; ``get_kid(other)``
+    returns ``(mean, std)`` against ``other``'s features -- a tensor, an array, or another KernelInceptionDistance (for example real
+    images' features computed once and kept with ``torch.save``) -- with the subsets' ix drawn from this set and iy from ``other``;
+    ``reset()`` drops the features.  ``kernel_kwargs``: ``degree``, ``gamma``, ``coef0`` and ``seed`` of ``calc_kid``."""
+
+    def __init__(self, num_subsets=100, subset_size=1000, input_transform=lambda x: x, device=torch.device("cpu"), **kernel_kwargs):
+        super().__init__()
+        unknown = set(kernel_kwargs) - set(KID_KERNEL_ARGS)
+        if unknown:
+            raise TypeError(f"unexpected keyword arguments {sorted(unknown)}; the kernel takes {', '.join(KID_KERNEL_ARGS)}")
+        self.num_subsets = num_subsets
+        self.subset_size = subset_size
+        self.kernel_kwargs = kernel_kwargs
+        self.input_transform = input_transform
+        self.device = device
+        self.model = self.load_model()
+        self._dev = _cuda_device(_op_device(device))
+        self._feats = []
+        self.count = 0
+
+    def load_model(self):
+        model = InceptionV3([3])
+        model.eval()
+        model.requires_grad_(False)
+        extractor = _FirstOutput(model)
+        if isinstance(self.device, (list, tuple)):
+            model.use_engine = False                           # under DataParallel, on torch, as InceptionStatistics
+            model.to(self.device[0])
+            return nn.DataParallel(extractor, device_ids=list(self.device))
+        return extractor.to(self.device)
+
+    def forward(self, x):
+        x = self.input_transform(x)
+        with torch.inference_mode():
+            net = self.model._module if isinstance(self.model, _FirstOutput) else None
+            if self._dev is not None and net is not None and net.native_eligible(x):
+                feats = net.forward_native(x, pooled=True)
+            else:
+                feats = self.model(x).flatten(1)
+            n = feats.shape[0]
+            if n == 0:
+                return
+            self._feats.append(feats.to(device=self._dev if self._dev is not None else "cpu", dtype=torch.float32))
+        self.count += n
+
+    @property
+    def features(self):
+        if len(self._feats) > 1:
+            self._feats = [torch.cat(self._feats)]
+        if not self._feats:
+            return torch.empty(0, IS_FEATURES, dtype=torch.float32, device=self._dev if self._dev is not None else "cpu")
+        return self._feats[0]
+
+    def get_kid(self, other):
+        other = other.features if isinstance(other, KernelInceptionDistance) else other
+        return calc_kid(self.features, other, self.num_subsets, self.subset_size,
+                        device=self._dev if self._dev is not None else "cpu", **self.kernel_kwargs)
+
+    def reset(self):
+        self._feats = []
+        self.count = 0
+
+
 __all__ = ["Manifold", "ManifoldBuilder", "calc_pr", "compute_distance", "to_uint8", "VGGFeatureExtractor",
            "InceptionV3", "InceptionStatistics", "get_precomputed", "calc_fd", "calculate_frechet_distance", "Evaluator",
-           "InceptionScore", "calc_is"]
+           "InceptionScore", "calc_is", "KernelInceptionDistance", "calc_kid"]

@@ -294,6 +294,21 @@ long long ddpm_is_score_scratch_bytes(int N, int C, int splits);
 int ddpm_is_score(const float* logits, int N, int C, long long ld, int splits, double* out, void* scratch, long long bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Kernel Inception Distance (Binkowski et al., 2018; the unbiased polynomial-kernel MMD^2 over subsets; kid.cuh).
+ * ddpm_kid  x fp32 [n1] rows of pitch ldx >= d, y fp32 [n2] rows of pitch ldy >= d (device, 4-byte aligned), 1 <= d <= 4096;
+ *           idx_host: a HOST array of S * 2 * m int32 indices, per subset s first ix (m rows of x) then iy (m rows of y), each in
+ *           range and distinct within its half (checked before any launch, then copied into the scratch on `stream`), 2 <= m <=
+ *           min(n1, n2).  With k(a, b) = (gamma a . b + coef0)^degree, 1 <= degree <= 8, out (fp64, S + 3 values):
+ *           out[s] = (sum_{i != j} k(x_i, x_j) + sum_{i != j} k(y_i, y_j)) / (m (m - 1)) - 2 sum_{i, j} k(x_i, y_j) / m^2 over the
+ *           rows of subset s, out[S] = their mean, out[S + 1] = their population std, out[S + 2] = status: 0, or 1 when a subset's
+ *           kernel sum is not finite (a non-finite feature in a drawn row, or an overflow); then out[S] and out[S + 1] are NaN.
+ *           Gram entries and sums in fp64 (DMMA), every reduction in a fixed order: the same rows give the same bits.
+ *           scratch: ddpm_kid_scratch_bytes(S, m) bytes, 16-byte aligned. */
+long long ddpm_kid_scratch_bytes(int S, int m);
+int ddpm_kid(const float* x, long long ldx, int n1, const float* y, long long ldy, int n2, int d, const int32_t* idx_host, int S, int m,
+             int degree, double gamma, double coef0, double* out, void* scratch, long long bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Low-level operators: GroupNorm(32, C, eps=1e-6) [+ SiLU] [+ dropout] (unet.py:18-20,83-84) and the bias column sums, with the
  * launch geometry the UNet engine's plans use (used by the parity tests of the engine itself).
  * Input = channel concat of two NHWC bf16 sources x0 [B][HW][C0] and x1 [B][HW][C1] (C1 = 0: one source).  C0 and C1 are
