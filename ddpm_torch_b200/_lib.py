@@ -198,6 +198,8 @@ def lib():
             "ddpm_knn_scratch_bytes": ([i32, i32, i32, i32], i64),
             "ddpm_knn_kth": ([vp, i32, i64, vp, i32, i64, i32, i32, vp, vp, i64, vp], i32),
             "ddpm_knn_cover": ([vp, i32, i64, vp, i32, i64, i32, vp, vp, vp, i64, vp], i32),
+            "ddpm_knn_count_scratch_bytes": ([i32, i32, i32], i64),
+            "ddpm_knn_count": ([vp, i32, i64, vp, i32, i64, i32, vp, vp, vp, i64, vp], i32),
             "ddpm_fid_stats_bytes": ([i32], i64),
             "ddpm_fid_stats_update": ([vp, i32, vp, i64, i64, vp], i32),
             "ddpm_fid_stats_finalize": ([vp, i32, i64, i32, vp, vp, vp], i32),
@@ -249,7 +251,7 @@ EXPORTS = ["ddpm_last_error", "ddpm_runtime_check", "ddpm_device_error_flag", "d
            "ddpm_unet_launches_per_forward", "ddpm_unet_launch_counts", "ddpm_opt_step", "ddpm_to_uint8_nhwc",
            "ddpm_unet_temb_layout", "ddpm_unet_temb_forward", "ddpm_unet_temb_backward",
            "ddpm_unet_image_layout", "ddpm_unet_image_forward", "ddpm_unet_image_backward",
-           "ddpm_knn_scratch_bytes", "ddpm_knn_kth", "ddpm_knn_cover",
+           "ddpm_knn_scratch_bytes", "ddpm_knn_kth", "ddpm_knn_cover", "ddpm_knn_count_scratch_bytes", "ddpm_knn_count",
            "ddpm_fid_stats_bytes", "ddpm_fid_stats_update", "ddpm_fid_stats_finalize", "ddpm_fid_distance_scratch_bytes",
            "ddpm_fid_distance", "ddpm_toy_num_params", "ddpm_toy_workspace_bytes", "ddpm_toy_forward", "ddpm_toy_train_forward",
            "ddpm_toy_backward", "ddpm_toy_train_backward", "ddpm_toy_sample",

@@ -455,7 +455,7 @@ static int knn_check_mat(const char* fn, const char* what, const void* x, long l
 
 long long ddpm_knn_scratch_bytes(int n_rows, int n_cols, int D, int kk) {
     const int rc = knn_check("ddpm_knn_scratch_bytes", n_rows, n_cols, D, kk);
-    return rc ? rc : (long long)knn_plan(n_rows, n_cols, D, kk).total;
+    return rc ? rc : (long long)knn_plan(kk > 0 ? KNN_KTH : KNN_COVER, n_rows, n_cols, D, kk).total;
 }
 
 // ManifoldBuilder.compute_kth (precision_recall.py:156-164): kth_out[i] = the (kk)-th smallest distance from row i to all columns.
@@ -468,11 +468,11 @@ int ddpm_knn_kth(const void* rows, int n_rows, long long ld_rows, const void* co
     if (!rc) rc = knn_check_mat(fn, "cols", cols, ld_cols, D);
     if (rc) return rc;
     if (!kth_out) return fail(-45, "%s: null kth_out", fn);
-    const size_t need = knn_plan(n_rows, n_cols, D, kk).total;
+    const size_t need = knn_plan(KNN_KTH, n_rows, n_cols, D, kk).total;
     if (!scratch || misaligned16(scratch) || bytes < (long long)need)
         return fail(-45, "%s: needs a 16-byte aligned scratch of ddpm_knn_scratch_bytes = %zu bytes (got %lld)", fn, need, bytes);
-    return knn_launch(static_cast<const __half*>(rows), n_rows, ld_rows, static_cast<const __half*>(cols), n_cols, ld_cols, D, kk,
-                      nullptr, kth_out, scratch, static_cast<cudaStream_t>(stream));
+    return knn_launch(KNN_KTH, static_cast<const __half*>(rows), n_rows, ld_rows, static_cast<const __half*>(cols), n_cols, ld_cols,
+                      D, kk, nullptr, kth_out, scratch, static_cast<cudaStream_t>(stream));
 }
 
 // calc_pr (precision_recall.py:177-206), one direction: covered[i] = any_j dist(probe i, support j) <= radii[j].
@@ -484,11 +484,34 @@ int ddpm_knn_cover(const void* probes, int n_probes, long long ld_p, const void*
     if (!rc) rc = knn_check_mat(fn, "support", support, ld_s, D);
     if (rc) return rc;
     if (!radii || !covered) return fail(-45, "%s: null radii or covered", fn);
-    const size_t need = knn_plan(n_probes, n_support, D, 0).total;
+    const size_t need = knn_plan(KNN_COVER, n_probes, n_support, D, 0).total;
     if (!scratch || misaligned16(scratch) || bytes < (long long)need)
         return fail(-45, "%s: needs a 16-byte aligned scratch of ddpm_knn_scratch_bytes(.., kk = 0) = %zu bytes (got %lld)", fn, need, bytes);
-    return knn_launch(static_cast<const __half*>(probes), n_probes, ld_p, static_cast<const __half*>(support), n_support, ld_s, D, 0,
-                      static_cast<const __half*>(radii), covered, scratch, static_cast<cudaStream_t>(stream));
+    return knn_launch(KNN_COVER, static_cast<const __half*>(probes), n_probes, ld_p, static_cast<const __half*>(support), n_support,
+                      ld_s, D, 0, static_cast<const __half*>(radii), covered, scratch, static_cast<cudaStream_t>(stream));
+}
+
+long long ddpm_knn_count_scratch_bytes(int n_probes, int n_support, int D) {
+    const int rc = knn_check("ddpm_knn_count_scratch_bytes", n_probes, n_support, D, 0);
+    return rc ? rc : (long long)knn_plan(KNN_COUNT, n_probes, n_support, D, 0).total;
+}
+
+// density of density/coverage (Naeem et al., 2020): counts[i] = #{j : dist(probe i, support j) < radii[j]}, strictly.
+int ddpm_knn_count(const void* probes, int n_probes, long long ld_p, const void* support, int n_support, long long ld_s, int D,
+                   const void* radii, int32_t* counts, void* scratch, long long bytes, void* stream) {
+    const char* fn = "ddpm_knn_count";
+    int rc = knn_check(fn, n_probes, n_support, D, 0);
+    if (!rc) rc = knn_check_mat(fn, "probes", probes, ld_p, D);
+    if (!rc) rc = knn_check_mat(fn, "support", support, ld_s, D);
+    if (rc) return rc;
+    if (!radii || !counts) return fail(-45, "%s: null radii or counts", fn);
+    if ((reinterpret_cast<uintptr_t>(radii) & 1) || (reinterpret_cast<uintptr_t>(counts) & 3))
+        return fail(-45, "%s: radii need 2-byte and counts 4-byte alignment", fn);
+    const size_t need = knn_plan(KNN_COUNT, n_probes, n_support, D, 0).total;
+    if (!scratch || misaligned16(scratch) || bytes < (long long)need)
+        return fail(-45, "%s: needs a 16-byte aligned scratch of ddpm_knn_count_scratch_bytes = %zu bytes (got %lld)", fn, need, bytes);
+    return knn_launch(KNN_COUNT, static_cast<const __half*>(probes), n_probes, ld_p, static_cast<const __half*>(support), n_support,
+                      ld_s, D, 0, static_cast<const __half*>(radii), counts, scratch, static_cast<cudaStream_t>(stream));
 }
 
 // ------------------------------------------------------------------------------------------------ Fréchet Inception Distance

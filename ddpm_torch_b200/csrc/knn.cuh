@@ -6,14 +6,15 @@
 //   na[i] = sum_d a[i,d]^2 in fp32 (k_knn_norms, fixed order);  d2[i,j] = max(0, (na[i] + nb[j]) - 2 <a_i, b_j>), the inner product
 //   on fp16 wgmma with fp32 accumulation;  kth[i] = fp16_rn(sqrt_rn(kk-th smallest d2[i, .]));  row i is covered iff
 //   exists j: fp16_rn(sqrt_rn(d2[i,j])) <= r[j].  fp16 o sqrt is monotone, so this is the reference's formula with exact distances
-//   in place of fp16 cdist.  Values only, no float atomics: two calls on the same inputs are bit-identical.
+//   in place of fp16 cdist.  The density of density/coverage (Naeem et al., 2020) counts instead, with a strict comparison:
+//   count[i] = #{j : fp16_rn(sqrt_rn(d2[i,j])) < r[j]}.  Values only, no atomics: two calls on the same inputs are bit-identical.
 //
 // Layout: the engine's warp-specialised persistent kernel.  Warpgroup 0 is the TMA producer, warpgroups 1-2 each own 64 rows of a
 // 128-row tile; 64-wide fp16 K slabs with 128-byte swizzle flow through a 4-stage mbarrier pipeline.  A work item is one row tile x a
-// contiguous range of 256-column tiles (a column split); the consumers keep per-row state (a register list of the kk smallest d2, or
-// a coverage flag) across all column tiles of the range, merge it over the quad of lanes that share a row, and write one entry per
-// (split, row) to scratch.  A small finalise kernel merges the splits.  Items run split-fastest, so CTAs that run together share
-// their row tile and walk the same column tiles (both operands are then mostly served from L2).
+// contiguous range of 256-column tiles (a column split); the consumers keep per-row state (a register list of the kk smallest d2, a
+// coverage flag or a count) across all column tiles of the range, merge it over the quad of lanes that share a row, and write one
+// entry per (split, row) to scratch.  A small finalise kernel merges the splits.  Items run split-fastest, so CTAs that run together
+// share their row tile and walk the same column tiles (both operands are then mostly served from L2).
 #pragma once
 #include <algorithm>
 #include <cuda_fp16.h>
@@ -29,16 +30,17 @@ constexpr int KNN_A_BYTES = 128 * 128;           // 128 rows x 64 fp16
 constexpr int KNN_B_BYTES = KNN_BN * 128;
 constexpr int KNN_STAGE_BYTES = KNN_A_BYTES + KNN_B_BYTES;
 constexpr int KNN_SMEM = 1024 /*align slack*/ + KNN_STAGES * KNN_STAGE_BYTES + 3 * KNN_BN * 4 + 2 * KNN_STAGES * 8;
-enum KnnMode { KNN_KTH = 0, KNN_COVER = 1 };
+enum KnnMode { KNN_KTH = 0, KNN_COVER = 1, KNN_COUNT = 2 };
 
 struct KnnParams {
     int n_rows, n_cols, kblocks;                 // kblocks = ceil(D / 64)
     int m_tiles, n_tiles, splits, per_split;     // item t: row tile t / splits, column tiles [s * per_split, ...) with s = t % splits
     int kk;                                      // kth: list length written per (split, row)
     const float* na; const float* nb;            // squared norms of the rows / columns
-    const __half* radii;                         // cover: r[n_cols]
+    const __half* radii;                         // cover, count: r[n_cols]
     float* part;                                 // kth: [splits][n_rows][kk]
     uint8_t* flags;                              // cover: [splits][n_rows]
+    int* counts;                                 // count: [splits][n_rows]
 };
 
 __device__ __forceinline__ void tma_load_2d(void* smem, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
@@ -60,7 +62,10 @@ __device__ __forceinline__ float knn_at(const float (&l)[KNN_MAX_K], int k) {
 }
 // the contract's coverage test of one distance: fp16_rn(sqrt_rn(d2)) <= r (compared as values, like the reference's fp16 `<=`)
 __device__ __forceinline__ bool knn_le(float d2, float r) { return __half2float(__float2half_rn(__fsqrt_rn(d2))) <= r; }
-// a d2 above this bound can never pass knn_le(d2, r): fp16_rn(sqrt(d2)) <= r needs sqrt(d2) below the next fp16 above r.
+// the density test of one distance: fp16_rn(sqrt_rn(d2)) < r (so a radius of 0, a negative radius or NaN contains nothing)
+__device__ __forceinline__ bool knn_lt(float d2, float r) { return __half2float(__float2half_rn(__fsqrt_rn(d2))) < r; }
+// a d2 above this bound can never pass knn_le(d2, r), nor therefore knn_lt: fp16_rn(sqrt(d2)) <= r needs sqrt(d2) below the next
+// fp16 above r.
 // (the 2^-10 margin covers the fp32 rounding of the square; -1 for a negative radius, which no distance can meet)
 __device__ __forceinline__ float knn_cover_bound(__half r) {
     const float rf = __half2float(r);
@@ -71,15 +76,16 @@ __device__ __forceinline__ float knn_cover_bound(__half r) {
     return up * up * (1.f + 0x1p-10f);
 }
 
+// The pass shared by every mode: main loop, column vectors and the per-mode epilogue.  The __global__ wrappers below pass their
+// __grid_constant__ parameters by reference, so the tensor maps are still read from parameter space.
 template <int MODE>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
-knn_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const KnnParams p) {
+__device__ __forceinline__ void knn_wgmma_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const KnnParams& p) {
     pdl_trigger();
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     float* s_nb = reinterpret_cast<float*>(smem + KNN_STAGES * KNN_STAGE_BYTES);   // [KNN_BN] nb of the current column tile
-    float* s_thr = s_nb + KNN_BN;                                                   // cover: knn_cover_bound(r)
-    float* s_rf = s_thr + KNN_BN;                                                   // cover: r as float
+    float* s_thr = s_nb + KNN_BN;                                                   // cover, count: knn_cover_bound(r)
+    float* s_rf = s_thr + KNN_BN;                                                   // cover, count: r as float
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(s_rf + KNN_BN);
     uint64_t* empty_bar = full_bar + KNN_STAGES;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -132,6 +138,7 @@ knn_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         float l0[KNN_MAX_K], l1[KNN_MAX_K];
         float thr0 = INFINITY, thr1 = INFINITY;
         bool cv0 = false, cv1 = false;
+        int n0 = 0, n1 = 0;
         if constexpr (MODE == KNN_KTH) {
 #pragma unroll
             for (int i = 0; i < KNN_MAX_K; ++i) { l0[i] = INFINITY; l1[i] = INFINITY; }
@@ -186,6 +193,21 @@ knn_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                     v = fmaxf(0.f, fmaf(-2.f, acc[4 * j + 3], na1 + nb2.y));
                     if (v < thr1) { knn_insert(l1, v); thr1 = knn_at(l1, k1); }
                 }
+            } else if constexpr (MODE == KNN_COUNT) {
+#pragma unroll
+                for (int j = 0; j < KNN_BN / 8; ++j) {
+                    const int c = 8 * j + 2 * q;
+                    const float2 nb2 = *reinterpret_cast<const float2*>(s_nb + c);
+                    const float2 th2 = *reinterpret_cast<const float2*>(s_thr + c);
+                    float v = fmaxf(0.f, fmaf(-2.f, acc[4 * j + 0], na0 + nb2.x));
+                    if (v <= th2.x && knn_lt(v, s_rf[c])) ++n0;
+                    v = fmaxf(0.f, fmaf(-2.f, acc[4 * j + 1], na0 + nb2.y));
+                    if (v <= th2.y && knn_lt(v, s_rf[c + 1])) ++n0;
+                    v = fmaxf(0.f, fmaf(-2.f, acc[4 * j + 2], na1 + nb2.x));
+                    if (v <= th2.x && knn_lt(v, s_rf[c])) ++n1;
+                    v = fmaxf(0.f, fmaf(-2.f, acc[4 * j + 3], na1 + nb2.y));
+                    if (v <= th2.y && knn_lt(v, s_rf[c + 1])) ++n1;
+                }
             } else {
 #pragma unroll
                 for (int j = 0; j < KNN_BN / 8; ++j) {
@@ -221,6 +243,14 @@ knn_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                     if (i < p.kk) { if (ok0) d0[i] = l0[i]; if (ok1) d1[i] = l1[i]; }
                 }
             }
+        } else if constexpr (MODE == KNN_COUNT) {
+            n0 += __shfl_xor_sync(0xffffffffu, n0, 1); n0 += __shfl_xor_sync(0xffffffffu, n0, 2);
+            n1 += __shfl_xor_sync(0xffffffffu, n1, 1); n1 += __shfl_xor_sync(0xffffffffu, n1, 2);
+            if (q == 0) {
+                int* d = p.counts + (size_t)sp * p.n_rows;
+                if (ok0) d[row0] = n0;
+                if (ok1) d[row1] = n1;
+            }
         } else {
             int f0 = cv0 ? 1 : 0, f1 = cv1 ? 1 : 0;
             f0 |= __shfl_xor_sync(0xffffffffu, f0, 1); f0 |= __shfl_xor_sync(0xffffffffu, f0, 2);
@@ -232,6 +262,17 @@ knn_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             }
         }
     }
+}
+
+template <int MODE>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+knn_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const KnnParams p) {
+    knn_wgmma_body<MODE>(tmA, tmB, p);
+}
+
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+knn_count_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const KnnParams p) {
+    knn_wgmma_body<KNN_COUNT>(tmA, tmB, p);
 }
 
 // squared row norms in fp32, one warp per row: lane l sums chunks l, l + 32, ... of 8 elements in order, then a fixed butterfly
@@ -281,6 +322,16 @@ __global__ void k_knn_cover_final(const uint8_t* flags, int splits, int n_rows, 
     out[row] = f;
 }
 
+// count: sum over the splits
+__global__ void k_knn_count_final(const int* counts, int splits, int n_rows, int* out) {
+    pdl_entry();
+    const int row = blockIdx.x * blockDim.x + threadIdx.x;
+    if (row >= n_rows) return;
+    int c = 0;
+    for (int s = 0; s < splits; ++s) c += counts[(size_t)s * n_rows + row];
+    out[row] = c;
+}
+
 // ------------------------------------------------------------------------------------------------ host side
 struct KnnPlan {
     int m_tiles = 0, n_tiles = 0, splits = 1, per_split = 0, kblocks = 0;
@@ -290,7 +341,7 @@ inline size_t knn_align(size_t n) { return (n + 255) & ~size_t(255); }
 // Column splits: the fewest waves of (row tile, column range) items over kPlanSms CTAs, counted in column tiles per CTA; among
 // equal counts the largest split up to max(16, SMs / row tiles), so that CTAs running together share a row tile.  Fixed by the
 // shape alone (kPlanSms, not the device), so the scratch size is too; the result does not depend on it.
-inline KnnPlan knn_plan(int n_rows, int n_cols, int D, int kk) {
+inline KnnPlan knn_plan(KnnMode mode, int n_rows, int n_cols, int D, int kk) {
     KnnPlan pl;
     pl.m_tiles = (n_rows + 127) / 128; pl.n_tiles = (n_cols + KNN_BN - 1) / KNN_BN; pl.kblocks = (D + 63) / 64;
     const int cap = std::min(pl.n_tiles, std::max(16, (kPlanSms + pl.m_tiles - 1) / pl.m_tiles));
@@ -305,7 +356,8 @@ inline KnnPlan knn_plan(int n_rows, int n_cols, int D, int kk) {
     pl.splits = (pl.n_tiles + pl.per_split - 1) / pl.per_split;   // no empty ranges
     pl.off_nb = knn_align((size_t)n_rows * 4);
     pl.off_part = pl.off_nb + knn_align((size_t)n_cols * 4);
-    const size_t part = kk > 0 ? (size_t)pl.splits * n_rows * kk * 4 : (size_t)pl.splits * n_rows;
+    const size_t entry = mode == KNN_KTH ? (size_t)kk * 4 : mode == KNN_COUNT ? 4 : 1;
+    const size_t part = (size_t)pl.splits * n_rows * entry;
     pl.total = pl.off_part + knn_align(part);
     return pl;
 }
@@ -325,18 +377,20 @@ inline int make_tmap_f16_2d(CUtensorMap* m, const void* ptr, int D, int rows, lo
     return 0;
 }
 
-// Both passes: norms of rows and columns, the wgmma pass, the finalise.  kk > 0: kth radii into out (fp16 [n_rows]);
-// kk == 0: coverage flags of the rows against radii (u8 [n_rows]).  Arguments are checked by the caller.
-inline int knn_launch(const __half* rows, int n_rows, long long ld_r, const __half* cols, int n_cols, long long ld_c, int D, int kk,
-                      const __half* radii, void* out, void* scratch, cudaStream_t st) {
-    const KnnPlan pl = knn_plan(n_rows, n_cols, D, kk);
+// Every pass: norms of rows and columns, the wgmma pass, the finalise.  KNN_KTH: kth radii into out (fp16 [n_rows]);
+// KNN_COVER: coverage flags of the rows against radii (u8 [n_rows]); KNN_COUNT: counts of the balls holding each row (int32
+// [n_rows]).  Arguments are checked by the caller.
+inline int knn_launch(KnnMode mode, const __half* rows, int n_rows, long long ld_r, const __half* cols, int n_cols, long long ld_c,
+                      int D, int kk, const __half* radii, void* out, void* scratch, cudaStream_t st) {
+    const KnnPlan pl = knn_plan(mode, n_rows, n_cols, D, kk);
     uint8_t* s = static_cast<uint8_t*>(scratch);
     KnnParams p;
     p.n_rows = n_rows; p.n_cols = n_cols; p.kblocks = pl.kblocks; p.m_tiles = pl.m_tiles; p.n_tiles = pl.n_tiles;
     p.splits = pl.splits; p.per_split = pl.per_split; p.kk = kk;
     p.na = reinterpret_cast<float*>(s); p.nb = reinterpret_cast<float*>(s + pl.off_nb); p.radii = radii;
-    p.part = kk > 0 ? reinterpret_cast<float*>(s + pl.off_part) : nullptr;
-    p.flags = kk > 0 ? nullptr : s + pl.off_part;
+    p.part = mode == KNN_KTH ? reinterpret_cast<float*>(s + pl.off_part) : nullptr;
+    p.flags = mode == KNN_COVER ? s + pl.off_part : nullptr;
+    p.counts = mode == KNN_COUNT ? reinterpret_cast<int*>(s + pl.off_part) : nullptr;
     CUtensorMap tA, tB;
     int rc = make_tmap_f16_2d(&tA, rows, D, n_rows, ld_r, 128);
     if (!rc) rc = make_tmap_f16_2d(&tB, cols, D, n_cols, ld_c, KNN_BN);
@@ -349,13 +403,14 @@ inline int knn_launch(const __half* rows, int n_rows, long long ld_r, const __ha
     DDPM_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     const int items = pl.m_tiles * pl.splits;
     const int ctas = std::max(1, std::min(items, sms));
-    auto kern = kk > 0 ? knn_wgmma_kernel<KNN_KTH> : knn_wgmma_kernel<KNN_COVER>;
+    auto kern = mode == KNN_KTH ? knn_wgmma_kernel<KNN_KTH> : mode == KNN_COVER ? knn_wgmma_kernel<KNN_COVER> : knn_count_kernel;
     DDPM_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, KNN_SMEM));
     launch_k(kern, ctas, GEMM_THREADS, KNN_SMEM, st, tA, tB, p);
     DDPM_CUDA_OK(cudaGetLastError());
     const unsigned g = (unsigned)((n_rows + 255) / 256);
-    if (kk > 0) launch_k(k_knn_kth_final, g, 256, 0, st, (const float*)p.part, pl.splits, n_rows, kk, static_cast<__half*>(out));
-    else launch_k(k_knn_cover_final, g, 256, 0, st, (const uint8_t*)p.flags, pl.splits, n_rows, static_cast<uint8_t*>(out));
+    if (mode == KNN_KTH) launch_k(k_knn_kth_final, g, 256, 0, st, (const float*)p.part, pl.splits, n_rows, kk, static_cast<__half*>(out));
+    else if (mode == KNN_COVER) launch_k(k_knn_cover_final, g, 256, 0, st, (const uint8_t*)p.flags, pl.splits, n_rows, static_cast<uint8_t*>(out));
+    else launch_k(k_knn_count_final, g, 256, 0, st, (const int*)p.counts, pl.splits, n_rows, static_cast<int*>(out));
     DDPM_CUDA_OK(cudaGetLastError());
     return 0;
 }

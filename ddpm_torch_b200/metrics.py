@@ -1,5 +1,6 @@
 """The evaluation metrics of ``ddpm_torch/metrics``: improved precision and recall (Kynkäänniemi et al., 2019) of
-``precision_recall.py`` with its k-NN half on the engine, FID (``fid_score.py``, ``__init__.py``'s ``Evaluator``) with its
+``precision_recall.py`` with its k-NN half on the engine, density and coverage (Naeem et al., 2020; ``calc_dc``, see its
+section) on the same real manifold, FID (``fid_score.py``, ``__init__.py``'s ``Evaluator``) with its
 statistics and Fréchet distance on the engine (see the FID section below), and the Inception Score (``InceptionScore``, ``calc_is``)
 and the Kernel Inception Distance (``KernelInceptionDistance``, ``calc_kid``; see their sections), which the reference does not have.
 
@@ -275,6 +276,94 @@ def calc_pr(manifold_1: Manifold, manifold_2: Manifold, row_batch_size: int, col
         return torch.cat(pred).to(torch.float32).mean()
 
     return coverage(f1, f2, k2), coverage(f2, f1, k1)
+
+
+# ================================================================================================ density and coverage
+# Naeem et al. (2020), "Reliable Fidelity and Diversity Metrics for Generative Models": with X the N real features, Y the M
+# generated ones, r_i the real manifold's fp16 radius (the k-th neighbour of X_i within X, X_i itself excluded:
+# ManifoldBuilder(nhood_size=k).kth) and d = fp16_rn(sqrt_rn(d2)) on the fp16 features as stored (the convention of calc_pr),
+#   density  = 1 / (k M) * sum_j #{i : d(Y_j, X_i) < r_i}      (may exceed 1)
+#   coverage = 1 / N * #{i : min_j d(X_i, Y_j) < r_i}.
+# Both comparisons are strict, unlike calc_pr's `<=`: a radius of 0 (duplicated real points), a negative radius or NaN holds
+# nothing; +inf holds every point whose fp16 distance is finite.  fp16 o sqrt is monotone, so coverage is decided by the nearest
+# generated point alone.
+# * CUDA ``device``: ``ddpm_knn_count`` (the k-NN GEMM with a counting epilogue, csrc/knn.cuh) gives the [M] counts and
+#   ``ddpm_knn_kth`` with kk = 1 (rows real, columns generated) the [N] nearest distances; only those come back to the host.
+# * CPU ``device``: the same recipe blockwise in torch, d2 in fp64 from the fp16 features, rounded to fp32, then fp32 sqrt and fp16,
+#   with no M x N matrix held.
+
+def _native_count(probes, support, radii, dev):
+    """``ddpm_knn_count`` on ``dev``'s current stream: int32 [n] counts of the balls (``support``, ``radii``) holding each probe,
+    as a CPU tensor."""
+    L = _lib.lib()
+    n, m, D = probes.shape[0], support.shape[0], probes.shape[1]
+    with torch.cuda.device(dev):
+        a, b = _device_rows(probes, dev), _device_rows(support, dev)
+        nbytes = L.ddpm_knn_count_scratch_bytes(n, m, D)
+        if nbytes < 0:
+            _lib.check(int(nbytes), "knn_count_scratch_bytes")
+        scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        r = radii.to(device=dev, dtype=torch.float16).contiguous()
+        out = torch.empty(n, dtype=torch.int32, device=dev)
+        _lib.check(L.ddpm_knn_count(a.data_ptr(), n, a.stride(0), b.data_ptr(), m, b.stride(0), D, r.data_ptr(), out.data_ptr(),
+                                    scratch.data_ptr(), nbytes, _lib.stream_ptr(dev)), "calc_dc")
+        return out.cpu()
+
+
+def _dc_host(y, x, radii, max_elems=1 << 22):
+    """The CPU recipe: (int64 [M] counts of the balls (x, radii) holding each row of y, fp16 [N] distance from each row of x to
+    its nearest row of y), one block of y rows against all of x at a time."""
+    x64 = x.detach().cpu().to(torch.float16).double()
+    nx = (x64 * x64).sum(1)
+    rf = radii.cpu().float()
+    counts = []
+    min_d2 = torch.full((x.shape[0],), float("inf"), dtype=torch.float64)
+    for yb in y.detach().cpu().to(torch.float16).split(max(1, max_elems // x.shape[0])):
+        y64 = yb.double()
+        d2 = ((y64 * y64).sum(1)[:, None] + nx[None, :] - 2.0 * (y64 @ x64.T)).clamp_min(0.0)
+        d = d2.float().sqrt().half().float()
+        counts.append((d < rf[None, :]).sum(1))
+        min_d2 = torch.minimum(min_d2, d2.min(0).values)
+    return torch.cat(counts), min_d2.float().sqrt().half()
+
+
+def calc_dc(manifold_1, manifold_2, nhood_size, device):
+    """Density and coverage ``(density, coverage)`` as Python floats, as defined in the section comment above.
+
+    ``manifold_1``: the generated set, a Manifold, a (features, kth) pair or a bare [M, D] tensor (its kth is not used).
+    ``manifold_2``: the real manifold, in any format calc_pr takes (a Manifold, the reference's namedtuple, a (features, kth)
+    pair).  ``nhood_size``: the k the real radii were built with; it divides the density, so it has no default.  ``device``: a
+    CUDA device (or a list, whose first entry is used) runs the native passes on its current stream; a CPU device the torch
+    recipe on the host.  ValueError for features that are not 2-D, a feature-dimension mismatch, an empty set,
+    ``nhood_size`` < 1 and radii whose length is not N."""
+    f1 = manifold_1 if isinstance(manifold_1, torch.Tensor) else _fields(manifold_1)[0]
+    f2, radii = _fields(manifold_2)
+    if radii is None:
+        raise ValueError("the real manifold needs its radii (kth); build it with ManifoldBuilder")
+    f1, f2, radii = torch.as_tensor(f1), torch.as_tensor(f2), torch.as_tensor(radii)
+    if f1.dim() != 2 or f2.dim() != 2:
+        raise ValueError(f"features must be [n, D], got {tuple(f1.shape)} and {tuple(f2.shape)}")
+    (m, D), n = f1.shape, f2.shape[0]
+    if f2.shape[1] != D:
+        raise ValueError(f"feature dimensions differ: {D} and {f2.shape[1]}")
+    if m == 0 or n == 0 or D == 0:
+        raise ValueError(f"density and coverage need non-empty sets (M = {m}, N = {n}, D = {D})")
+    if int(nhood_size) != nhood_size or nhood_size < 1:
+        raise ValueError(f"nhood_size must be an integer >= 1, got {nhood_size}")
+    if tuple(radii.shape) != (n,):
+        raise ValueError(f"the real manifold needs one radius per real feature: {tuple(radii.shape)} radii for N = {n}")
+    radii = radii.to(torch.float16)
+    dev = _cuda_device(_op_device(device))
+    if dev is None:
+        counts, nearest = _dc_host(f1, f2, radii)
+    else:
+        with torch.cuda.device(dev):
+            y, x = _device_rows(f1, dev)[:, :D], _device_rows(f2, dev)[:, :D]     # copied once, read by both passes
+            counts = _native_count(y, x, radii, dev)
+            nearest = _native("calc_dc", x, y, 1, None, dev)
+    total = int(counts.to(torch.int64).sum())
+    covered = int((nearest.float() < radii.cpu().float()).sum())
+    return total / (int(nhood_size) * m), covered / n
 
 
 # ================================================================================================ FID (fid_score.py)
@@ -943,6 +1032,6 @@ class KernelInceptionDistance(nn.Module):
         self.count = 0
 
 
-__all__ = ["Manifold", "ManifoldBuilder", "calc_pr", "compute_distance", "to_uint8", "VGGFeatureExtractor",
+__all__ = ["Manifold", "ManifoldBuilder", "calc_pr", "calc_dc", "compute_distance", "to_uint8", "VGGFeatureExtractor",
            "InceptionV3", "InceptionStatistics", "get_precomputed", "calc_fd", "calculate_frechet_distance", "Evaluator",
            "InceptionScore", "calc_is", "KernelInceptionDistance", "calc_kid"]

@@ -191,14 +191,21 @@ long long ddpm_conv_scratch_bytes(const ddpm_conv_desc* d);
  *                including row i itself when rows == cols; kk = nhood_size + 1 in 1..16 and kk <= n_cols.
  * ddpm_knn_cover (calc_pr, :177-206, one direction): covered u8 [n_probes] = 1 iff some support j has
  *                fp16_rn(sqrt_rn(d2[i,j])) <= radii[j] (fp16 [n_support]), else 0.
- * scratch: caller-owned, 16-byte aligned, ddpm_knn_scratch_bytes(n_rows, n_cols, D, kk) bytes (kk = 0 for ddpm_knn_cover); no
- * initialisation needed.  No allocation, no synchronisation, graph-capturable; results are bit-identical from call to call.  Every
- * argument error is refused before any device work. */
+ * ddpm_knn_count (density of density/coverage, Naeem et al. 2020): counts int32 [n_probes] = #{ j : fp16_rn(sqrt_rn(d2[i,j])) <
+ *                radii[j] }, a strict comparison: a radius of 0, a negative radius or NaN holds nothing, +inf holds every point
+ *                whose fp16 distance is finite.  radii 2-byte and counts 4-byte aligned.
+ * scratch: caller-owned, 16-byte aligned, ddpm_knn_scratch_bytes(n_rows, n_cols, D, kk) bytes (kk = 0 for ddpm_knn_cover;
+ * ddpm_knn_count_scratch_bytes(n_probes, n_support, D) for ddpm_knn_count); no initialisation needed.  No allocation, no
+ * synchronisation, no atomics, graph-capturable; results are bit-identical from call to call.  Every argument error is refused
+ * before any device work. */
 long long ddpm_knn_scratch_bytes(int n_rows, int n_cols, int D, int kk);
 int ddpm_knn_kth(const void* rows, int n_rows, long long ld_rows, const void* cols, int n_cols, long long ld_cols, int D, int kk,
                  void* kth_out, void* scratch, long long bytes, void* stream);
 int ddpm_knn_cover(const void* probes, int n_probes, long long ld_p, const void* support, int n_support, long long ld_s, int D,
                    const void* radii, uint8_t* covered, void* scratch, long long bytes, void* stream);
+long long ddpm_knn_count_scratch_bytes(int n_probes, int n_support, int D);
+int ddpm_knn_count(const void* probes, int n_probes, long long ld_p, const void* support, int n_support, long long ld_s, int D,
+                   const void* radii, int32_t* counts, void* scratch, long long bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Fréchet Inception Distance (ddpm_torch/metrics/fid_score.py), fp64 throughout, on the fp64 tensor cores (DMMA) where it is a
