@@ -180,6 +180,8 @@ def lib():
             "ddpm_bpd_setup": ([vp, i32, vp], i32),
             "ddpm_bpd_reset": ([vp, i32, vp], i32),
             "ddpm_bpd_step": ([vp, vp, vp, i32, vp, vp, vp], i32),
+            "ddpm_bpd_terms_scratch_bytes": ([i32, i32, i32], i64),
+            "ddpm_bpd_terms_run": ([i32, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp, i64, vp, vp, vp], i32),
             "ddpm_unet_grad_chunks": ([vp, i32, C.POINTER(i64), C.POINTER(i64)], i32),
             "ddpm_unet_wait_grad_chunk": ([vp, i32, vp], i32),
             "ddpm_unet_plan_stats": ([vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32),
@@ -247,7 +249,8 @@ EXPORTS = ["ddpm_last_error", "ddpm_runtime_check", "ddpm_device_error_flag", "d
            "ddpm_unet_flat_elems", "ddpm_unet_graph_epoch", "ddpm_unet_workspace_bytes", "ddpm_unet_plan", "ddpm_unet_repack",
            "ddpm_unet_forward", "ddpm_unet_backward", "ddpm_unet_backward_ex", "ddpm_unet_backward_launches", "ddpm_train_forward", "ddpm_train_backward",
            "ddpm_sampler_setup", "ddpm_sampler_reset", "ddpm_sampler_step", "ddpm_sampler_step_pred",
-           "ddpm_bpd_setup", "ddpm_bpd_reset", "ddpm_bpd_step", "ddpm_unet_grad_chunks", "ddpm_unet_wait_grad_chunk", "ddpm_unet_plan_stats",
+           "ddpm_bpd_setup", "ddpm_bpd_reset", "ddpm_bpd_step",
+           "ddpm_bpd_terms_scratch_bytes", "ddpm_bpd_terms_run", "ddpm_unet_grad_chunks", "ddpm_unet_wait_grad_chunk", "ddpm_unet_plan_stats",
            "ddpm_unet_launches_per_forward", "ddpm_unet_launch_counts", "ddpm_opt_step", "ddpm_to_uint8_nhwc",
            "ddpm_unet_temb_layout", "ddpm_unet_temb_forward", "ddpm_unet_temb_backward",
            "ddpm_unet_image_layout", "ddpm_unet_image_forward", "ddpm_unet_image_backward",

@@ -1093,18 +1093,44 @@ int ddpm_bpd_step(ddpm_unet* h, const float* x0, const float* noise, int clip_de
     e.qs_pro = QsamplePro{};
     e.bpd_epi = BpdEpi{};
     if (rc) return rc;
-    const int nbi = (HW + 255) / 256;
-    if (!fused) {
-        switch (Cout) {
-            case 1: launch_k(k_bpd_tail<1>, e.B * nbi, 256, 0, st, (const float*)eps, bp, HW); break;
-            case 2: launch_k(k_bpd_tail<2>, e.B * nbi, 256, 0, st, (const float*)eps, bp, HW); break;
-            case 3: launch_k(k_bpd_tail<3>, e.B * nbi, 256, 0, st, (const float*)eps, bp, HW); break;
-            default: launch_k(k_bpd_tail<4>, e.B * nbi, 256, 0, st, (const float*)eps, bp, HW); break;
-        }
-        DDPM_CUDA_OK(cudaGetLastError());
-    }
-    launch_k(k_bpd_finalize, 1, 256, 0, st, (const float*)part, nbi, e.B, (float)(Cout * HW), (const float*)cc, T, losses, mses);
-    DDPM_CUDA_OK(cudaGetLastError());
+    if (!fused) DDPM_CUDA_OK((cudaError_t)launch_bpd_tail(Cout, st, eps, bp, e.B, HW));
+    DDPM_CUDA_OK((cudaError_t)launch_bpd_finalize(st, part, e.B, Cout, HW, cc, T, losses, mses));
+    return 0;
+}
+// scratch: the coefficient row (kBpdRow + 1 floats, padded to 64 bytes), then the block partials f32 [bpd_blocks(B, H*W)][2]
+static long long bpd_terms_scratch(int B, int H, int W) { return 64 + (long long)bpd_blocks(B, H * W) * 2 * 4; }
+static int bpd_terms_check_dims(const char* fn, int B, int H, int W) {
+    if (B < 1 || H < 1 || W < 1) return fail(-30, "%s: need B, H, W >= 1", fn);
+    if ((long long)H * W > INT_MAX || (long long)B * (((long long)H * W + 255) / 256) > INT_MAX)
+        return fail(-30, "%s: B x H x W too large for one launch", fn);
+    return 0;
+}
+long long ddpm_bpd_terms_scratch_bytes(int B, int H, int W) {
+    const int rc = bpd_terms_check_dims("ddpm_bpd_terms_scratch_bytes", B, H, W);
+    return rc ? rc : bpd_terms_scratch(B, H, W);
+}
+int ddpm_bpd_terms_run(int route, const float* src, const float* bias, const float* x0, const float* xt, const float* row_host, int clip,
+                       int B, int C, int H, int W, int T, void* scratch, long long scratch_bytes, float* losses, float* mses, void* stream) {
+    const char* fn = "ddpm_bpd_terms_run";
+    if (route != 0 && route != 1) return fail(-30, "%s: route must be 0 (k_bpd_tail over eps) or 1 (k_out_gather over tap sums)", fn);
+    if (C < 1 || C > (route == 0 ? 4 : 3)) return fail(-30, "%s: C must be in 1..%d on route %d (got %d)", fn, route == 0 ? 4 : 3, route, C);
+    int rc = bpd_terms_check_dims(fn, B, H, W);
+    if (rc) return rc;
+    if (!src || !x0 || !xt || !row_host || !scratch || !losses || !mses || (route == 1 && !bias)) return fail(-30, "%s: null buffer", fn);
+    if (T <= 0 || T > (1 << 24)) return fail(-30, "%s: T must be in 1..2^24 (the step index travels as a float)", fn);
+    const float ti = row_host[kBpdRow];
+    if (!(ti >= 0.f && ti < (float)T && ti == floorf(ti))) return fail(-30, "%s: step index row[%d] must be an integer in [0, T)", fn, kBpdRow);
+    if (misaligned16(scratch)) return fail(-30, "%s: scratch must be 16-byte aligned", fn);
+    if (scratch_bytes < bpd_terms_scratch(B, H, W))
+        return fail(-30, "%s: scratch of %lld bytes, need %lld", fn, scratch_bytes, bpd_terms_scratch(B, H, W));
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    float* cc = static_cast<float*>(scratch);
+    float* part = reinterpret_cast<float*>(static_cast<uint8_t*>(scratch) + 64);
+    DDPM_CUDA_OK(cudaMemcpyAsync(cc, row_host, (kBpdRow + 1) * sizeof(float), cudaMemcpyHostToDevice, st));
+    const BpdEpi bp{x0, xt, cc, part, clip ? 1 : 0};
+    if (route == 0) DDPM_CUDA_OK((cudaError_t)launch_bpd_tail(C, st, src, bp, B, H * W));
+    else DDPM_CUDA_OK((cudaError_t)launch_out_gather(C, 0, st, src, bias, nullptr, B, H, W, PsampleEpi{nullptr, nullptr, nullptr, 0, nullptr}, bp));
+    DDPM_CUDA_OK((cudaError_t)launch_bpd_finalize(st, part, B, C, H * W, cc, T, losses, mses));
     return 0;
 }
 int ddpm_opt_step(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, float* ema_shadow, long long n,

@@ -81,6 +81,39 @@ static inline int launch_gn_prep(const GnApply& a, int Bn, cudaStream_t st) {
     launch_k(k_gn_prep, Bn, C < 256 ? C : 256, 0, st, a);
     return (int)cudaGetLastError();
 }
+// ------------------------------------------------------------------ bits/dim launches
+// Shared by ddpm_bpd_step (through the plan's out_conv.2.gather op or the tail after the forward) and the bits/dim operator of
+// the C ABI (ddpm_bpd_terms_run), so that both launch the same kernels on the same grid: one 256-thread block per 256 pixels
+// of one image, blocks never straddling images (kernels_simt.cuh).
+static inline int bpd_blocks(int Bn, int HW) { return Bn * ((HW + 255) / 256); }
+// k_out_gather<Cout>, Cout 1..3: the bits/dim grid when bp.part is set, else the caller's grid-stride grid nblk
+static inline int launch_out_gather(int Cout, int nblk, cudaStream_t st, const float* T, const float* bias, float* out, int Bn, int Hn,
+                                    int Wn, const PsampleEpi& ps, const BpdEpi& bp) {
+    const int g = bp.part ? bpd_blocks(Bn, Hn * Wn) : nblk;
+    switch (Cout) {
+        case 1: launch_k(k_out_gather<1>, g, 256, 0, st, T, bias, out, Bn, Hn, Wn, ps, bp); break;
+        case 2: launch_k(k_out_gather<2>, g, 256, 0, st, T, bias, out, Bn, Hn, Wn, ps, bp); break;
+        default: launch_k(k_out_gather<3>, g, 256, 0, st, T, bias, out, Bn, Hn, Wn, ps, bp); break;
+    }
+    return (int)cudaGetLastError();
+}
+// k_bpd_tail<Cout>, Cout 1..4, over eps f32 [Bn][Cout][HW]
+static inline int launch_bpd_tail(int Cout, cudaStream_t st, const float* eps, const BpdEpi& bp, int Bn, int HW) {
+    const int g = bpd_blocks(Bn, HW);
+    switch (Cout) {
+        case 1: launch_k(k_bpd_tail<1>, g, 256, 0, st, eps, bp, HW); break;
+        case 2: launch_k(k_bpd_tail<2>, g, 256, 0, st, eps, bp, HW); break;
+        case 3: launch_k(k_bpd_tail<3>, g, 256, 0, st, eps, bp, HW); break;
+        default: launch_k(k_bpd_tail<4>, g, 256, 0, st, eps, bp, HW); break;
+    }
+    return (int)cudaGetLastError();
+}
+// k_bpd_finalize over the bpd_blocks(Bn, HW) partials: losses / mses [Bn][T], column coef[kBpdRow]
+static inline int launch_bpd_finalize(cudaStream_t st, const float* part, int Bn, int Cout, int HW, const float* coef, int T,
+                                      float* losses, float* mses) {
+    launch_k(k_bpd_finalize, 1, 256, 0, st, part, (HW + 255) / 256, Bn, (float)(Cout * HW), coef, T, losses, mses);
+    return (int)cudaGetLastError();
+}
 // dropout is armed per call by a non-zero seed
 static inline void gn_arm_dropout(float& drop_p, unsigned long long& seed, unsigned long long run_seed) { seed = run_seed; if (!seed) drop_p = 0.f; }
 // k_gn_bwd_reduce + k_gn_bwd_apply; the apply pass also accumulates the column sums of dx when any of the cs pointers is set

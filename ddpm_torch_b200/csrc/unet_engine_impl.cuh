@@ -293,7 +293,7 @@ inline int UnetEngine::plan(int B_, int H_, int W_, bool train_, bool dry_) {
     xt_off = alloc(img_elems * 4); eps_off = alloc((size_t)B * Cout * H * W * 4);
     tbuf_off = alloc((size_t)B * 8); coefcur_off = alloc(64); counter_off = alloc(64);
     deps_off = alloc((size_t)B * Cout * H * W * 4);
-    bpd_part_off = alloc((size_t)B * ((H * W + 255) / 256) * 2 * 4);
+    bpd_part_off = alloc((size_t)bpd_blocks(B, H * W) * 2 * 4);
 
     // ---- zero the per-forward accumulators
     { uint8_t* z = ws + zero_fwd_off; const size_t n = zero_fwd_bytes;
@@ -637,16 +637,8 @@ inline int UnetEngine::plan(int B_, int H_, int W_, bool train_, bool dry_) {
             } else push(fwd_ops, "out_conv.2", fl, [](cudaStream_t) { return 0; });
             gather_fused_tail = true;             // the sampler's alpha/beta update (ddpm_sampler_step) or the bits/dim terms
                                                   // (ddpm_bpd_step) ride in this kernel
-            const int nblk_bpd = Bn * ((Hn * Wn + 255) / 256);
             push(fwd_ops, "out_conv.2.gather", 0, [=](cudaStream_t st) {
-                const BpdEpi bpe = self->bpd_epi;
-                const int g = bpe.part ? nblk_bpd : nblk;
-                switch (Cout) {
-                    case 1: launch_k(k_out_gather<1>, g, 256, 0, st, T, bo, self->eps_dst, Bn, Hn, Wn, self->ps_epi, bpe); break;
-                    case 2: launch_k(k_out_gather<2>, g, 256, 0, st, T, bo, self->eps_dst, Bn, Hn, Wn, self->ps_epi, bpe); break;
-                    default: launch_k(k_out_gather<3>, g, 256, 0, st, T, bo, self->eps_dst, Bn, Hn, Wn, self->ps_epi, bpe); break;
-                }
-                return (int)cudaGetLastError(); });
+                return launch_out_gather(Cout, nblk, st, T, bo, self->eps_dst, Bn, Hn, Wn, self->ps_epi, self->bpd_epi); });
         } else
         push(fwd_ops, "out_conv.2", fl, [=](cudaStream_t st) {
             switch (Cout) {

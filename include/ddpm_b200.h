@@ -458,6 +458,19 @@ int ddpm_sampler_step_pred(ddpm_unet* h, float* x, const float* z, uint64_t seed
 int ddpm_bpd_setup(ddpm_unet* h, int T, const float* coef_host);
 int ddpm_bpd_reset(ddpm_unet* h, int first_step, void* stream);
 int ddpm_bpd_step(ddpm_unet* h, const float* x0, const float* noise, int clip_denoised, float* losses, float* mses, void* stream);
+/* The bits/dim terms of one step alone, on caller buffers: what ddpm_bpd_step launches after the UNet forward, with eps given
+ * (the same launch helpers, so the same kernels on the same grid of B * ceil(H*W / 256) blocks of 256 threads) — an
+ * operator-level test of the engine.
+ *   route 0: k_bpd_tail<C>, C in 1..4, over src = eps f32 [B][C][H][W] (bias unused);
+ *   route 1: the bits/dim path of k_out_gather<C>, C in 1..3, over src = the out_conv.2 tap sums T f32 [B*H*W][32] (tap t,
+ *            channel c at t*C + c), eps = bias[c] + the sum of the in-bounds taps; bias f32 [C];
+ *   then k_bpd_finalize: losses[b][ti] / mses[b][ti] of f32 [B][T], no other column written.
+ * x0, xt f32 [B][C][H][W].  row_host: HOST pointer to kBpdRow + 1 = 10 floats, one ddpm_bpd_setup row followed by the step
+ * index ti (an integer in [0, T), T <= 2^24), copied into scratch ahead of the launches as k_sampler_prep copies it.
+ * scratch: >= ddpm_bpd_terms_scratch_bytes(B, H, W) bytes, 16-byte aligned.  Every argument is checked before any launch. */
+long long ddpm_bpd_terms_scratch_bytes(int B, int H, int W);
+int ddpm_bpd_terms_run(int route, const float* src, const float* bias, const float* x0, const float* xt, const float* row_host, int clip,
+                       int B, int C, int H, int W, int T, void* scratch, long long scratch_bytes, float* losses, float* mses, void* stream);
 /* Data-parallel training (train.py:110 DDP, utils/train.py:149-153): the backward pass finishes the flat gradient buffer in
  * contiguous CHUNKS, level group by level group, and records a CUDA event per chunk.  grad_chunks returns their number and
  * fills lo/hi (element offsets into the flat buffer, in completion order; together they tile it exactly); wait_grad_chunk makes
