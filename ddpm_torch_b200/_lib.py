@@ -228,6 +228,7 @@ def lib():
             "ddpm_kid": ([vp, i64, i32, vp, i64, i32, i32, vp, i32, i32, i32, C.c_double, C.c_double, vp, vp, i64, vp], i32),
             "ddpm_toy_num_params": ([vp], i64),
             "ddpm_toy_workspace_bytes": ([vp, i64, i32], i64),
+            "ddpm_toy_ws_layout": ([vp, i64, i32, C.POINTER(i64 * 8), C.POINTER(i32), C.POINTER(i64), C.POINTER(i64)], i32),
             "ddpm_toy_forward": ([vp, vp, vp, vp, i64, vp, i32, vp, i64, vp], i32),
             "ddpm_toy_train_forward": ([vp, vp, vp, vp, vp, vp, vp, i64, vp, vp, i64, vp], i32),
             "ddpm_toy_backward": ([vp, vp, vp, vp, i64, vp, vp, vp, i64, vp], i32),
@@ -256,7 +257,7 @@ EXPORTS = ["ddpm_last_error", "ddpm_runtime_check", "ddpm_device_error_flag", "d
            "ddpm_unet_image_layout", "ddpm_unet_image_forward", "ddpm_unet_image_backward",
            "ddpm_knn_scratch_bytes", "ddpm_knn_kth", "ddpm_knn_cover", "ddpm_knn_count_scratch_bytes", "ddpm_knn_count",
            "ddpm_fid_stats_bytes", "ddpm_fid_stats_update", "ddpm_fid_stats_finalize", "ddpm_fid_distance_scratch_bytes",
-           "ddpm_fid_distance", "ddpm_toy_num_params", "ddpm_toy_workspace_bytes", "ddpm_toy_forward", "ddpm_toy_train_forward",
+           "ddpm_fid_distance", "ddpm_toy_num_params", "ddpm_toy_workspace_bytes", "ddpm_toy_ws_layout", "ddpm_toy_forward", "ddpm_toy_train_forward",
            "ddpm_toy_backward", "ddpm_toy_train_backward", "ddpm_toy_sample",
            "ddpm_inception_num_params", "ddpm_inception_param_info", "ddpm_inception_conv_info", "ddpm_inception_packed_bytes", "ddpm_inception_pack",
            "ddpm_inception_workspace_bytes", "ddpm_inception_forward", "ddpm_inception_conv_scratch_bytes", "ddpm_inception_conv_run",

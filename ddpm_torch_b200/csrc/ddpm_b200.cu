@@ -1416,6 +1416,19 @@ long long ddpm_toy_workspace_bytes(const ddpm_toy_cfg* cfg, long long rows, int 
     return (long long)toy_ws_layout(cfg->mid_features, cfg->in_features, cfg->num_layers, rows, training ? 1 : 0).total;
 }
 
+int ddpm_toy_ws_layout(const ddpm_toy_cfg* cfg, long long rows, int training, long long* off, int* slots, long long* P, long long* Pp) {
+    if (int rc = toy_check("ddpm_toy_ws_layout", cfg, rows)) return rc;
+    if (!off || !slots || !P || !Pp) return fail(-47, "ddpm_toy_ws_layout: null output");
+    const int tr = training ? 1 : 0;
+    const ToyWs w = toy_ws_layout(cfg->mid_features, cfg->in_features, cfg->num_layers, rows, tr);
+    const size_t o[8] = {w.E, w.h, w.u, w.x, w.out, w.dE, w.part, w.total};
+    for (int i = 0; i < 8; ++i) off[i] = (long long)o[i];
+    const ToyLayout lay(cfg->mid_features, cfg->in_features, cfg->num_layers);
+    *slots = tr ? toy_grid((int)rows, TOY_BWD_CTAS) : 0;
+    *P = lay.P; *Pp = lay.Pp;
+    return 0;
+}
+
 int ddpm_toy_forward(const ddpm_toy_cfg* cfg, const ddpm_toy_params* p, const float* x, const long long* t, long long B, float* out,
                      int training, void* ws, long long ws_bytes, void* stream) {
     const char* fn = "ddpm_toy_forward";

@@ -566,6 +566,11 @@ typedef struct {
 } ddpm_toy_params;
 long long ddpm_toy_num_params(const ddpm_toy_cfg* cfg);
 long long ddpm_toy_workspace_bytes(const ddpm_toy_cfg* cfg, long long rows, int training);
+/* Operator-level: the workspace layout the launches use, for tests that read the saves.  off[8] = byte offsets of E f32 [rows][M],
+ * h f32 [L+1][rows][M], u f32 [L][rows][M], x_t f32 [rows][D], out f32 [rows][D], dE f32 [rows][M], the partial slots f32
+ * [slots][Pp] (flat parameters() layout, P used) and the total; the training-only entries are 0 and slots = 0 when training = 0.
+ * Arguments are checked as in ddpm_toy_workspace_bytes. */
+int ddpm_toy_ws_layout(const ddpm_toy_cfg* cfg, long long rows, int training, long long* off, int* slots, long long* P, long long* Pp);
 int ddpm_toy_forward(const ddpm_toy_cfg* cfg, const ddpm_toy_params* p, const float* x, const long long* t, long long B, float* out,
                      int training, void* ws, long long ws_bytes, void* stream);
 int ddpm_toy_train_forward(const ddpm_toy_cfg* cfg, const ddpm_toy_params* p, const float* x0, const long long* t, const float* noise,

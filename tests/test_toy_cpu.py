@@ -94,7 +94,7 @@ def test_cpu_model_raises_at_call_time():
 
 def test_exports_and_refusals():
     L = _lib.lib()
-    for name in ("ddpm_toy_num_params", "ddpm_toy_workspace_bytes", "ddpm_toy_forward", "ddpm_toy_train_forward",
+    for name in ("ddpm_toy_num_params", "ddpm_toy_workspace_bytes", "ddpm_toy_ws_layout", "ddpm_toy_forward", "ddpm_toy_train_forward",
                  "ddpm_toy_backward", "ddpm_toy_train_backward", "ddpm_toy_sample"):
         assert name in _lib.EXPORTS
         getattr(L, name)
