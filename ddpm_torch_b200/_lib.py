@@ -214,6 +214,7 @@ def lib():
             "ddpm_inception_pack": ([vp, vp, vp], i32),
             "ddpm_inception_workspace_bytes": ([i32, i32, i32, i32, i32], i64),
             "ddpm_inception_forward": ([vp, vp, i32, i32, i32, i32, i32, i32, C.POINTER(vp * 4), vp, vp, i64, vp], i32),
+            "ddpm_inception_forward_ex": ([vp, vp, i32, i32, i32, i32, i32, i32, C.POINTER(vp * 4), vp, vp, vp, i64, vp], i32),
             "ddpm_inception_conv_scratch_bytes": ([C.POINTER(IncConvDesc)], i64),
             "ddpm_inception_conv_run": ([C.POINTER(IncConvDesc), vp], i32),
             "ddpm_inception_pool_run": ([i32, vp, i32, i32, i32, i32, vp, i32, i32, vp], i32),
@@ -260,7 +261,8 @@ EXPORTS = ["ddpm_last_error", "ddpm_runtime_check", "ddpm_device_error_flag", "d
            "ddpm_fid_distance", "ddpm_toy_num_params", "ddpm_toy_workspace_bytes", "ddpm_toy_ws_layout", "ddpm_toy_forward", "ddpm_toy_train_forward",
            "ddpm_toy_backward", "ddpm_toy_train_backward", "ddpm_toy_sample",
            "ddpm_inception_num_params", "ddpm_inception_param_info", "ddpm_inception_conv_info", "ddpm_inception_packed_bytes", "ddpm_inception_pack",
-           "ddpm_inception_workspace_bytes", "ddpm_inception_forward", "ddpm_inception_conv_scratch_bytes", "ddpm_inception_conv_run",
+           "ddpm_inception_workspace_bytes", "ddpm_inception_forward", "ddpm_inception_forward_ex", "ddpm_inception_conv_scratch_bytes",
+           "ddpm_inception_conv_run",
            "ddpm_inception_pool_run", "ddpm_inception_input_run",
            "ddpm_is_fc_packed_bytes", "ddpm_is_fc_pack", "ddpm_is_logits_workspace_bytes", "ddpm_is_logits",
            "ddpm_is_score_scratch_bytes", "ddpm_is_score", "ddpm_kid_scratch_bytes", "ddpm_kid"]

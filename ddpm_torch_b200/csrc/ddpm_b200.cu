@@ -639,9 +639,9 @@ long long ddpm_inception_workspace_bytes(int N, int H, int W, int resize, int la
     return (long long)b;
 }
 
-int ddpm_inception_forward(const void* packed, const float* x, int N, int H, int W, int resize, int normalize, int last_block,
-                           float* const outs[4], float* pooled, void* ws, long long ws_bytes, void* stream) {
-    const char* fn = "ddpm_inception_forward";
+// ddpm_inception_forward with sFID's spatial tap (spatial: null, or [N][h w 7] fp32 of Mixed_6d, which needs last_block >= 2)
+static int inc_forward(const char* fn, const void* packed, const float* x, int N, int H, int W, int resize, int normalize,
+                       int last_block, float* const outs[4], float* pooled, float* spatial, void* ws, long long ws_bytes, void* stream) {
     if (int rc = inc_check_shape(fn, N, H, W, resize, last_block)) return rc;
     if (normalize != 0 && normalize != 1) return fail(-47, "%s: normalize must be 0 or 1 (got %d)", fn, normalize);
     if (!packed || misaligned(packed, 256)) return fail(-47, "%s: packed must be a non-null, 256-byte aligned buffer", fn);
@@ -650,6 +650,9 @@ int ddpm_inception_forward(const void* packed, const float* x, int N, int H, int
         if (outs[b] && (b > last_block || misaligned(outs[b], 4)))
             return fail(-47, "%s: outs[%d] must be null or a 4-byte aligned buffer of a block <= last_block", fn, b);
     if (pooled && misaligned(pooled, 4)) return fail(-47, "%s: pooled must be 4-byte aligned", fn);
+    if (spatial && (last_block < 2 || misaligned(spatial, 4)))
+        return fail(-47, "%s: spatial must be null or a 4-byte aligned buffer, with last_block >= 2 (Mixed_6d is in block 2; got %d)",
+                    fn, last_block);
     IncWalk w;
     const char* why = nullptr;
     const size_t need = inc_workspace(N, H, W, resize, last_block, w, why);
@@ -659,7 +662,7 @@ int ddpm_inception_forward(const void* packed, const float* x, int N, int H, int
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     uint8_t* p = static_cast<uint8_t*>(ws);
     for (int b = 0; b < IncWalk::NBUF; ++b) { w.buf[b] = reinterpret_cast<float*>(p); p += inc_al256((size_t)w.need[b] * 4); }
-    w.dry = false; w.packed = static_cast<const float*>(packed); w.st = st;
+    w.dry = false; w.packed = static_cast<const float*>(packed); w.st = st; w.spatial = spatial;
     w.err = inc_input_launch(x, N, H, W, resize, normalize, w.buf[IncWalk::X], st);
     inc_walk(w, H, W, resize, last_block, [&](int b, int buf, int h, int wd, int C) {
         if (!w.ok()) return;
@@ -675,6 +678,18 @@ int ddpm_inception_forward(const void* packed, const float* x, int N, int H, int
             w.err = launch_k(k_inc_gap, dim3(inc_grid((long long)N * C)), dim3(256), 0, st, src, N, (int)hw, C, pooled, C);
     });
     return w.err == cudaSuccess ? 0 : fail(-20, "%s: launch failed: %s", fn, cudaGetErrorString(w.err));
+}
+
+int ddpm_inception_forward(const void* packed, const float* x, int N, int H, int W, int resize, int normalize, int last_block,
+                           float* const outs[4], float* pooled, void* ws, long long ws_bytes, void* stream) {
+    return inc_forward("ddpm_inception_forward", packed, x, N, H, W, resize, normalize, last_block, outs, pooled, nullptr, ws,
+                       ws_bytes, stream);
+}
+
+int ddpm_inception_forward_ex(const void* packed, const float* x, int N, int H, int W, int resize, int normalize, int last_block,
+                              float* const outs[4], float* pooled, float* spatial, void* ws, long long ws_bytes, void* stream) {
+    return inc_forward("ddpm_inception_forward_ex", packed, x, N, H, W, resize, normalize, last_block, outs, pooled, spatial, ws,
+                       ws_bytes, stream);
 }
 
 // the table entry a test conv stands for: any of the network's kernel shapes, with the caller's channel counts

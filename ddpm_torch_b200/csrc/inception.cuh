@@ -13,7 +13,8 @@
 // batch it arrives in or on the call.
 //
 // Everything else is plain SIMT: the input kernel (bilinear resize to 299 x 299 as F.interpolate(align_corners=False) computes it,
-// 2x - 1, NCHW -> NHWC with 4 channels), the 3 x 3 pools, the global average and the NHWC -> NCHW copy of a block output.
+// 2x - 1, NCHW -> NHWC with 4 channels), the 3 x 3 pools, the global average, the NHWC -> NCHW copy of a block output and, on
+// request, the gather of sFID's spatial features (channels 0..6 of Mixed_6d's output) while that output is still in its buffer.
 #pragma once
 #include <climits>
 #include <string>
@@ -329,6 +330,18 @@ __global__ void k_inc_nchw(const float* __restrict__ x, int N, int HW, int C, fl
     }
 }
 
+// sFID's spatial features (Nash et al., 2021, as the guided-diffusion evaluator reads mixed_6/conv:0[..., :7]): channels
+// [0, INC_SPATIAL_C) of NHWC [N][HW][C] -> rows out[n][p * INC_SPATIAL_C + c], p = h W + w, i.e. TensorFlow's NHWC flatten.  Pixel
+// q = n HW + p of the input lands at q * INC_SPATIAL_C + c of the output, so the output is written in order, one float per thread.
+constexpr int INC_SPATIAL_C = 7;
+__global__ void k_sfid_gather(const float* __restrict__ x, long long pixels, int C, float* __restrict__ out) {
+    pdl_entry();
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < pixels * INC_SPATIAL_C; i += (long long)gridDim.x * blockDim.x) {
+        const long long q = i / INC_SPATIAL_C;
+        out[i] = x[q * C + (i - q * INC_SPATIAL_C)];
+    }
+}
+
 // ------------------------------------------------------------------------------------------------ host side: the layer table
 // split: the network's first conv reads the input kernel's 12-channel split image (see k_inc_input) and is packed to match
 struct IncConv { int cin, cout, kh, kw, stride, ph, pw; std::string name; bool split = false; };
@@ -508,6 +521,7 @@ struct IncWalk {
     const char* bad = nullptr;                 // a shape the network cannot take (dry)
     int step = 0;                              // convs launched so far
     int (*layout)[4] = nullptr;                // dry, optional: per conv {c_off, C_total, writes the trunk (A / B), step}
+    float* spatial = nullptr;                  // optional: sFID's [N][H W INC_SPATIAL_C] features of Mixed_6d (see spatial_tap)
 
     bool ok() const { return err == cudaSuccess && bad == nullptr; }
     void use(int b, int H, int W, int C) {
@@ -538,6 +552,12 @@ struct IncWalk {
         } else if (ok()) {
             err = inc_pool_launch(kind, buf[src], N, H, W, C, buf[dst], c_off, C_total, st);
         }
+    }
+    // buffer `src` [H][W][C] holds Mixed_6d's output: gather sFID's features into `spatial` (nothing when it is null)
+    void spatial_tap(int src, int H, int W, int C) {
+        if (dry || !spatial || !ok()) return;
+        const long long pixels = (long long)N * H * W;
+        err = launch_k(k_sfid_gather, dim3(inc_grid(pixels * INC_SPATIAL_C)), dim3(256), 0, st, buf[src], pixels, C, spatial);
     }
 };
 
@@ -576,13 +596,16 @@ inline void inc_walk(IncWalk& w, int H, int W, int resize, int last_block, Emit&
     w.conv(i + 1, cur, h, wd, T0, 0, 64); w.conv(i + 2, T0, h, wd, T1, 0, 96); w.conv(i + 3, T1, h, wd, nxt, 384, 768);
     w.pool(INC_MAX3_S2, cur, h, wd, 288, nxt, 480, 768, h2, w2);
     std::swap(cur, nxt); h = ho; wd = wo; i += 4;
-    for (int c7 : {128, 160, 160, 192}) {                                // Mixed_6b..6e (C blocks)
+    const int c7s[4] = {128, 160, 160, 192};
+    for (int k = 0; k < 4; ++k) {                                        // Mixed_6b..6e (C blocks)
+        const int c7 = c7s[k];
         w.conv(i + 1, cur, h, wd, T0, 0, c7); w.conv(i + 2, T0, h, wd, T1, 0, c7); w.conv(i + 3, T1, h, wd, nxt, 192, 768);
         w.conv(i + 4, cur, h, wd, T0, 0, c7); w.conv(i + 5, T0, h, wd, T1, 0, c7); w.conv(i + 6, T1, h, wd, T0, 0, c7);
         w.conv(i + 7, T0, h, wd, T1, 0, c7); w.conv(i + 8, T1, h, wd, nxt, 384, 768);
         w.conv(i, cur, h, wd, nxt, 0, 768);
         w.pool(INC_AVG3_S1, cur, h, wd, 768, T2, 0, 768, ho, wo); w.conv(i + 9, T2, h, wd, nxt, 576, 768);
         std::swap(cur, nxt); i += 10;
+        if (k == 2) w.spatial_tap(cur, h, wd, 768);                     // Mixed_6d, before Mixed_7a overwrites this buffer
     }
     emit(2, cur, h, wd, 768);
     if (last_block == 2 || !w.ok()) return;

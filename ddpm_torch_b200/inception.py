@@ -2,6 +2,7 @@
 building blocks.  On an sm_90 device, with no gradient wanted and BatchNorm in eval mode, ``InceptionV3.forward`` runs on the
 engine (``ddpm_inception_forward``: TF32 tensor-core convolutions with BatchNorm folded in, csrc/inception.cuh); everything
 else (CPU, autograd, training-mode BatchNorm, ``DataParallel`` replicas, other dtypes) runs the torch modules below.
+``forward(x, spatial=True)`` also returns sFID's spatial features (``spatial_features``) from the same pass, on either route.
 
 The FID network differs from torchvision's ImageNet Inception-v3 in three places, all reproduced here:
   * 1008 classes (its ``fc`` is part of the checkpoint; only the Inception Score uses it, as ``InceptionV3.fc_weight``);
@@ -186,11 +187,14 @@ class InceptionV3(nn.Module):
         _lib.check(L.ddpm_inception_pack(raw.data_ptr(), self._packed.data_ptr(), _lib.stream_ptr(dev)), "inception_pack")
         self._packed_key = key
 
-    def forward_native(self, inp, pooled=False):
+    def forward_native(self, inp, pooled=False, spatial=False):
         """The engine's forward of ``inp`` (see ``native_eligible``): the requested blocks' outputs, NCHW fp32 as ``forward``
-        returns them; with ``pooled`` instead the [N, C] global average of the last needed block (InceptionStatistics)."""
+        returns them; with ``pooled`` instead the [N, C] global average of the last needed block (InceptionStatistics).  With
+        ``spatial`` the return value is a pair: that result and sFID's [N, 7 h w] features (``spatial_features``), gathered by
+        the engine from Mixed_6d's output in the same pass."""
         dev = inp.device
         L = _lib.lib()
+        self._check_spatial(spatial)
         with torch.cuda.device(dev):
             self._repack_if_needed(dev)
             x = inp.contiguous()
@@ -212,26 +216,59 @@ class InceptionV3(nn.Module):
                     h, w = _block_hw(H, W, self.resize_input, b)
                     res.append(torch.empty(N, _BLOCK_CHANNELS[b], h, w, dtype=torch.float32, device=dev))
                     outs[b] = res[-1].data_ptr()
-            _lib.check(L.ddpm_inception_forward(self._packed.data_ptr(), x.data_ptr(), N, H, W, int(self.resize_input),
-                                                int(self.normalize_input), last, C.byref(outs),
-                                                None if feats is None else feats.data_ptr(), self._ws.data_ptr(), self._ws.numel(),
-                                                _lib.stream_ptr(dev)), "InceptionV3")
-        return feats if pooled else res
+            sp = None
+            if spatial:
+                h, w = _block_hw(H, W, self.resize_input, 2)
+                sp = torch.empty(N, h * w * SPATIAL_CHANNELS, dtype=torch.float32, device=dev)
+            _lib.check(L.ddpm_inception_forward_ex(self._packed.data_ptr(), x.data_ptr(), N, H, W, int(self.resize_input),
+                                                   int(self.normalize_input), last, C.byref(outs),
+                                                   None if feats is None else feats.data_ptr(),
+                                                   None if sp is None else sp.data_ptr(), self._ws.data_ptr(), self._ws.numel(),
+                                                   _lib.stream_ptr(dev)), "InceptionV3")
+        out = feats if pooled else res
+        return (out, sp) if spatial else out
 
-    def forward(self, inp):
+    def _check_spatial(self, spatial):
+        if spatial and self.last_needed_block < 2:
+            raise ValueError("spatial features come from Mixed_6d, in block 2; this module stops at block "
+                             f"{self.last_needed_block}")
+
+    def forward(self, inp, spatial=False):
+        """The requested blocks' outputs; with ``spatial`` a pair of those and sFID's [N, 7 h w] features
+        (``spatial_features`` of Mixed_6d's output), from the same pass."""
+        self._check_spatial(spatial)
         if self.native_eligible(inp):
-            return self.forward_native(inp)
+            return self.forward_native(inp, spatial=spatial)
         x = inp
         if self.resize_input:
             x = F.interpolate(x, size=(299, 299), mode="bilinear", align_corners=False)
         if self.normalize_input:
             x = 2 * x - 1
-        out = []
+        out, sp = [], None
         for i, block in enumerate(self.blocks):
-            x = block(x)
+            if spatial and i == 2:
+                # module by module rather than through a hook, so that DataParallel replicas return the features too
+                for j, m in enumerate(block):
+                    x = m(x)
+                    if j == _MIXED_6D:
+                        sp = spatial_features(x)
+            else:
+                x = block(x)
             if i in self.output_blocks:
                 out.append(x)
-        return out
+        return (out, sp) if spatial else out
+
+
+def spatial_features(mixed_6d):
+    """sFID's spatial features (Nash et al., 2021) from Mixed_6d's NCHW output [N, 768, h, w]: channels [0, 7), which are
+    its branch1x1 after BatchNorm and ReLU (the first slice of the block's torch.cat), flattened in TensorFlow's NHWC order,
+    feature (y w + x) 7 + c: [N, 7 h w], 2023 features at 299 x 299.
+
+    This follows the guided-diffusion evaluator (Dhariwal & Nichol, 2021), which reads ``mixed_6/conv:0[..., :7]`` from the
+    TensorFlow 2015 Inception graph.  That ``mixed_6`` is ``Mixed_6d`` (``mixed_3`` is ``Mixed_6a``; ``mixed_4``..``mixed_7``
+    are ``6b``..``6e``) and that ``mixed_6/conv:0`` is the post-ReLU output of its 1x1 branch is assumed, not verified: the
+    values are meant to be comparable to ADM's sFID but have not been checked against it."""
+    return mixed_6d[:, :SPATIAL_CHANNELS].permute(0, 2, 3, 1).reshape(mixed_6d.shape[0], -1)
 
 
 _ENGINE_BLOCK = {"Conv2d_1a_3x3": "blocks.0.0", "Conv2d_2a_3x3": "blocks.0.1", "Conv2d_2b_3x3": "blocks.0.2",
@@ -239,6 +276,8 @@ _ENGINE_BLOCK = {"Conv2d_1a_3x3": "blocks.0.0", "Conv2d_2a_3x3": "blocks.0.1", "
                  **{f"Mixed_{m}": f"blocks.2.{i}" for i, m in enumerate(("5b", "5c", "5d", "6a", "6b", "6c", "6d", "6e"))},
                  **{f"Mixed_{m}": f"blocks.3.{i}" for i, m in enumerate(("7a", "7b", "7c"))}}
 _BLOCK_CHANNELS = (64, 192, 768, 2048)
+_MIXED_6D = 6                                    # its position in block 2
+SPATIAL_CHANNELS = 7                             # sFID keeps channels [0, 7) of Mixed_6d
 
 
 def _block_hw(H, W, resize, block):

@@ -1,7 +1,8 @@
 """The evaluation metrics of ``ddpm_torch/metrics``: improved precision and recall (Kynkäänniemi et al., 2019) of
 ``precision_recall.py`` with its k-NN half on the engine, density and coverage (Naeem et al., 2020; ``calc_dc``, see its
 section) on the same real manifold, FID (``fid_score.py``, ``__init__.py``'s ``Evaluator``) with its
-statistics and Fréchet distance on the engine (see the FID section below), and the Inception Score (``InceptionScore``, ``calc_is``)
+statistics and Fréchet distance on the engine (see the FID section below; sFID's spatial statistics come from the same pass with
+``InceptionStatistics(spatial=True)``), and the Inception Score (``InceptionScore``, ``calc_is``)
 and the Kernel Inception Distance (``KernelInceptionDistance``, ``calc_kid``; see their sections), which the reference does not have.
 
 Public names, signatures and defaults are the reference's: ``Manifold``, ``ManifoldBuilder``, ``calc_pr``,
@@ -379,9 +380,10 @@ def calc_dc(manifold_1, manifold_2, nhood_size, device):
 # features handed to adaptive_avg_pool2d for activation_dim != 2048 (InceptionStatistics.forward), and the empty last batch of
 # Evaluator.eval when the batch size divides the total.
 
-from .inception import InceptionV3, FID_WEIGHTS_URL  # noqa: E402
+from .inception import InceptionV3, FID_WEIGHTS_URL, SPATIAL_CHANNELS  # noqa: E402
 
 IMAGE_RES = 299
+SPATIAL_DIM = 17 * 17 * SPATIAL_CHANNELS      # sFID's features per image: Mixed_6d is 17 x 17 at 299 x 299
 FID_STATUS = {1: "a non-finite input", 2: "sigma1 (mean1's covariance) is not positive semi-definite",
               3: "sigma2 (mean2's covariance) is not positive semi-definite",
               4: "the eigen-solve of sigma1 did not converge", 5: "the eigen-solve of L^T sigma2 L did not converge"}
@@ -394,29 +396,43 @@ class InceptionStatistics(nn.Module):
     On a CUDA ``device`` (or the first device of a list, where Inception runs under ``DataParallel`` as upstream) the statistics
     live in the native fp64 state on that device; on the CPU they follow the reference's per-batch ``np.cov`` and merge.
     ``get_statistics()`` returns numpy fp64 ``(mean, cov)`` with cov divided by ``count - 1``; ``running_mean`` /
-    ``running_var`` are the population values (read-only)."""
+    ``running_var`` are the population values (read-only).
 
-    def __init__(self, input_transform=lambda x: x, activation_dim=2048, device=torch.device("cpu")):
+    With ``spatial=True`` every ``forward`` also folds sFID's 2023 spatial features (``inception.spatial_features``: channels
+    0..6 of Mixed_6d's output at 17 x 17, NHWC order) into a second set of statistics, from the same Inception pass, and
+    ``get_spatial_statistics()`` returns them like ``get_statistics()``.  sFID is then
+    ``calc_fd(*gen.get_spatial_statistics(), *real.get_spatial_statistics())``.  The features follow the guided-diffusion
+    evaluator's ``mixed_6/conv:0[..., :7]``; that TensorFlow tensor is assumed to be this one, which has not been verified, so
+    the values are meant to be comparable to ADM's sFID but have not been checked against it.  ``activation_dim`` 64 and 192
+    stop before Mixed_6d and refuse ``spatial=True``."""
+
+    def __init__(self, input_transform=lambda x: x, activation_dim=2048, device=torch.device("cpu"), spatial=False):
         super().__init__()
+        if spatial and InceptionV3.BLOCK_INDEX_BY_DIM.get(activation_dim, 3) < 2:
+            raise ValueError(f"spatial=True needs Mixed_6d, which activation_dim {activation_dim} stops before (use 768 or 2048)")
         self.input_transform = input_transform
         self.activation_dim = activation_dim
         self.device = device
+        self.spatial = bool(spatial)
         self.model = self.load_model()
         self._dev = _cuda_device(_op_device(device))
         self.count = 0
+        self._dims = (activation_dim, SPATIAL_DIM) if self.spatial else (activation_dim,)
         if self._dev is not None:
-            nbytes = _lib.lib().ddpm_fid_stats_bytes(activation_dim)
-            _lib.check(0 if nbytes > 0 else int(nbytes), "fid_stats_bytes")
-            self._state = torch.zeros(nbytes, dtype=torch.uint8, device=self._dev)
+            self._states = []
+            for D in self._dims:
+                nbytes = _lib.lib().ddpm_fid_stats_bytes(D)
+                _lib.check(0 if nbytes > 0 else int(nbytes), "fid_stats_bytes")
+                self._states.append(torch.zeros(nbytes, dtype=torch.uint8, device=self._dev))
         else:
-            self._mean = np.zeros((activation_dim,), dtype=np.float64)
-            self._var = np.zeros((activation_dim, activation_dim), dtype=np.float64)
+            self._moments = [(np.zeros((D,), dtype=np.float64), np.zeros((D, D), dtype=np.float64)) for D in self._dims]
+            self._mean, self._var = self._moments[0]
 
     def load_model(self):
         model = InceptionV3([InceptionV3.BLOCK_INDEX_BY_DIM[self.activation_dim]])
         model.eval()
         model.requires_grad_(False)
-        extractor = _FirstOutput(model)
+        extractor = _FirstOutput(model, spatial=self.spatial)
         if isinstance(self.device, (list, tuple)):
             model.use_engine = False                           # under DataParallel, on torch, as upstream
             model.to(self.device[0])
@@ -428,10 +444,14 @@ class InceptionStatistics(nn.Module):
         with torch.inference_mode():
             net = self.model._module if isinstance(self.model, _FirstOutput) else None
             if self._dev is not None and net is not None and net.native_eligible(x):
-                # the engine's global average of the last block, [N, D] rows fed to the statistics as they are
-                self._fold(net.forward_native(x, pooled=True))
+                # the engine's global average of the last block, [N, D] rows fed to the statistics as they are (and with
+                # spatial, the engine's [N, 2023] spatial features of the same pass)
+                out = net.forward_native(x, pooled=True, spatial=self.spatial)
+                self._fold(*(out if self.spatial else (out,)))
                 return
             act = self.model(x)
+            if self.spatial:
+                act, sp = act
             # Upstream pools after .cpu().numpy(), and adaptive_avg_pool2d refuses a numpy array: activation_dim 64 / 192 / 768
             # raised TypeError.  Pooled here, on the features' own device, before they leave it.
             if act.shape[2] != 1 or act.shape[3] != 1:
@@ -440,37 +460,45 @@ class InceptionStatistics(nn.Module):
         n = act.shape[0]
         if n == 0:
             return
+        feats = (act, sp) if self.spatial else (act,)
         if self._dev is not None:
-            self._fold(act)
+            self._fold(*feats)
             return
-        act = act.cpu().numpy()
+        for (m, v), f in zip(self._moments, feats):
+            self._merge(m, v, f.cpu().numpy())
+        self.count += n
+
+    def _merge(self, m, v, act):
+        """fid_score.py:116-135: the batch's np.cov (ddof 0) merged into the running mean m and population covariance v."""
+        n = act.shape[0]
         mean = np.mean(act, axis=0, dtype=np.float64)
         var = np.cov(act, rowvar=False, ddof=0, dtype=np.float64)
         alpha = n / (self.count + n)
         if self.count == 0:
-            self._mean += mean
-            self._var += var
+            m += mean
+            v += var
         else:
-            diff = mean - self._mean
-            self._mean += alpha * diff
-            self._var += alpha * (var - self._var)
-            self._var += alpha * (1 - alpha) * np.outer(diff, diff)
-        self.count += n
+            diff = mean - m
+            m += alpha * diff
+            v += alpha * (var - v)
+            v += alpha * (1 - alpha) * np.outer(diff, diff)
 
-    def _fold(self, act):
-        n = act.shape[0]
-        feats = act.to(device=self._dev, dtype=torch.float32).contiguous()
+    def _fold(self, *feats):
+        """Each [n, D] batch into its native state (pool3, then the spatial features)."""
+        n = feats[0].shape[0]
         with torch.cuda.device(self._dev):
-            _lib.check(_lib.lib().ddpm_fid_stats_update(self._state.data_ptr(), self.activation_dim, feats.data_ptr(), n,
-                                                        feats.stride(0), _lib.stream_ptr(self._dev)), "InceptionStatistics")
+            for state, D, act in zip(self._states, self._dims, feats):
+                f = act.to(device=self._dev, dtype=torch.float32).contiguous()
+                _lib.check(_lib.lib().ddpm_fid_stats_update(state.data_ptr(), D, f.data_ptr(), n, f.stride(0),
+                                                            _lib.stream_ptr(self._dev)), "InceptionStatistics")
         self.count += n
 
-    def _native_stats(self, ddof):
-        D = self.activation_dim
+    def _native_stats(self, ddof, which=0):
+        D = self._dims[which]
         with torch.cuda.device(self._dev):
             mean = torch.empty(D, dtype=torch.float64, device=self._dev)
             cov = torch.empty(D, D, dtype=torch.float64, device=self._dev)
-            _lib.check(_lib.lib().ddpm_fid_stats_finalize(self._state.data_ptr(), D, self.count, ddof, mean.data_ptr(),
+            _lib.check(_lib.lib().ddpm_fid_stats_finalize(self._states[which].data_ptr(), D, self.count, ddof, mean.data_ptr(),
                                                           cov.data_ptr(), _lib.stream_ptr(self._dev)), "InceptionStatistics")
             return mean.cpu().numpy(), cov.cpu().numpy()
 
@@ -496,21 +524,38 @@ class InceptionStatistics(nn.Module):
             return self._native_stats(1)
         return self._mean.copy(), self._var.copy() * self.count / (self.count - 1)
 
+    def get_spatial_statistics(self):
+        """sFID's statistics (``spatial=True``): numpy fp64 ``(mean [2023], cov [2023, 2023])``, cov divided by ``count - 1``."""
+        if not self.spatial:
+            raise RuntimeError("get_spatial_statistics needs InceptionStatistics(spatial=True)")
+        assert self.count > 1, "Count must be greater than 1!"
+        if self._dev is not None:
+            return self._native_stats(1, which=1)
+        m, v = self._moments[1]
+        return m.copy(), v.copy() * self.count / (self.count - 1)
+
     def reset(self):
         if self._dev is not None:
-            self._state.zero_()
+            for s in self._states:
+                s.zero_()
         else:
-            self._mean.fill(0)
-            self._var.fill(0)
+            for m, v in self._moments:
+                m.fill(0)
+                v.fill(0)
         self.count = 0
 
 
 class _FirstOutput(nn.Module):
-    def __init__(self, module):
+    """The module's first output; with ``spatial`` the pair (first output, sFID's spatial features)."""
+    def __init__(self, module, spatial=False):
         super().__init__()
         self._module = module
+        self.spatial = spatial
 
     def forward(self, x):
+        if self.spatial:
+            out, sp = self._module(x, spatial=True)
+            return out[0], sp
         return self._module(x)[0]
 
 

@@ -248,6 +248,13 @@ int ddpm_fid_distance(const double* mu1, const double* sigma1, const double* mu2
  *                         [N][192][.][.], [N][768][.][.], [N][2048][1][1].  pooled (may be null) <- [N][C] global average of block
  *                         last_block (for block 3 the same values as outs[3]).  ws: ddpm_inception_workspace_bytes(N, H, W,
  *                         resize, last_block) bytes, 256-byte aligned; that call refuses (< 0) an input too small for the block.
+ *                         The same as ddpm_inception_forward_ex with spatial = null.
+ * ddpm_inception_forward_ex  ddpm_inception_forward plus sFID's spatial features (Nash et al., 2021).  spatial (may be null) <-
+ *                         [N][h w 7] fp32: channels 0..6 of Mixed_6d's output (its branch1x1 after BatchNorm and ReLU), h x w its
+ *                         block-2 size (17 x 17 at 299 x 299), flattened in TensorFlow's NHWC order, feature (y w + x) 7 + c.
+ *                         The guided-diffusion evaluator reads mixed_6/conv:0[..., :7]; that this is the same tensor is assumed,
+ *                         not verified.  A non-null spatial needs last_block >= 2 and 4-byte alignment.  Same workspace; with
+ *                         spatial = null it launches exactly what ddpm_inception_forward launches.
  * ddpm_inception_conv_run one conv of the network's kind: x NHWC fp32 [N][H][W][Cin rounded up to 4] (16-byte aligned), raw
  *                         weights and BatchNorm vectors as in the state_dict, out channels [c_off, c_off + Cout) of NHWC
  *                         [N][Ho][Wo][C_total] (Cout, c_off, C_total even); scratch: ddpm_inception_conv_scratch_bytes(d).
@@ -272,6 +279,8 @@ int ddpm_inception_pack(const float* raw, void* packed, void* stream);
 long long ddpm_inception_workspace_bytes(int N, int H, int W, int resize, int last_block);
 int ddpm_inception_forward(const void* packed, const float* x, int N, int H, int W, int resize, int normalize, int last_block,
                            float* const outs[4], float* pooled, void* ws, long long ws_bytes, void* stream);
+int ddpm_inception_forward_ex(const void* packed, const float* x, int N, int H, int W, int resize, int normalize, int last_block,
+                              float* const outs[4], float* pooled, float* spatial, void* ws, long long ws_bytes, void* stream);
 long long ddpm_inception_conv_scratch_bytes(const ddpm_inception_conv_desc* d);
 int ddpm_inception_conv_run(const ddpm_inception_conv_desc* d, void* stream);
 int ddpm_inception_pool_run(int kind, const float* x, int N, int H, int W, int C, float* out, int c_off, int C_total, void* stream);
